@@ -346,10 +346,10 @@ struct Engine::Impl {
                         &sym_d[1], &sym_d[2], &outbuf, &emit_desc, &err_flag};
     for (DevBuf* d : shared) d->st = lane[0].stream;
     CK(cudaFuncSetAttribute(k_match, cudaFuncAttributeMaxDynamicSharedMemorySize, kMatchSmemBytes));
-    {
+    for (const void* k : {(const void*)k_iterate<2>, (const void*)k_iterate<kWideWarps>}) {
       cudaFuncAttributes fa;
-      CK(cudaFuncGetAttributes(&fa, k_iterate));
-      CK(cudaFuncSetAttribute(k_iterate, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - (int)fa.sharedSizeBytes));
+      CK(cudaFuncGetAttributes(&fa, k));
+      CK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - (int)fa.sharedSizeBytes));
     }
     g_log.start();
   }
@@ -383,6 +383,7 @@ struct Engine::Impl {
     std::vector<uint32_t> order;
     uint64_t nkeys = 0, npos = 0;
     bool any_parse = false;
+    bool any_optimal = false;  // a segment runs the iterated optimal parse (not only fixed-tree parses)
   };
 
   void build_layout(const std::vector<ParseRange>& r, Layout& L) {
@@ -407,6 +408,7 @@ struct Engine::Impl {
       L.nkeys += s.nkeys;
       L.npos += s.npos;
       if (s.mode != 0) L.any_parse = true;
+      if (s.mode == 1) L.any_optimal = true;
       for (uint32_t f = 0; f < s.nkeys; f += kKeyChunk) L.kw.push_back({(uint32_t)i, f});
       for (uint32_t f = 0; f < s.npos; f += kMatchPosPerCta) L.pw.push_back({(uint32_t)i, f});
     }
@@ -758,12 +760,22 @@ void Engine::parse_common(const std::vector<ParseRange>& ranges, ParseResult& ou
       // has a scheduler partition of its own (a partition mate costs the chain ~20% of its speed)
       // A batch of only a few blocks (the giants of stage C) takes whole SMs: with 188 KB of padding
       // no kernel that uses shared memory can move in beside the chain.
-      static const unsigned static_smem = [] { cudaFuncAttributes fa; CK(cudaFuncGetAttributes(&fa, k_iterate)); return (unsigned)fa.sharedSizeBytes; }();
+      // Those whole-SM launches of optimal parses run the wide form of k_iterate: its other six warps take part
+      // in trace-back and follow-path.  ZOPFLI_B200_WIDE=0 / 1 forces the two-warp / wide form for every launch.
+      static const unsigned static_smem = [] { cudaFuncAttributes fa; CK(cudaFuncGetAttributes(&fa, k_iterate<2>)); return (unsigned)fa.sharedSizeBytes; }();
       static const unsigned pad_many = [] { const char* e = getenv("ZOPFLI_B200_ITER_PAD"); return e ? (unsigned)atoi(e) : 56u * 1024u - static_smem; }();
       static const unsigned pad_few = [] { const char* e = getenv("ZOPFLI_B200_ITER_PAD_FEW"); return e ? (unsigned)atoi(e) : 222u * 1024u - static_smem; }();
-      unsigned pad = ns <= 64 ? pad_few : pad_many;
+      static const int wide_env = [] { const char* e = getenv("ZOPFLI_B200_WIDE"); return e ? atoi(e) : -1; }();
+      const bool few = ns <= 64;
+      const bool wide = wide_env < 0 ? few && L.any_optimal : wide_env != 0;
+      unsigned pad = few ? pad_few : pad_many;
       if (pad < sizeof(IterDyn)) pad = (unsigned)sizeof(IterDyn);  // the integer window's tables live in the dynamic part
-      k_iterate<<<(unsigned)ns, 64, pad, l.stream>>>(b, l.order.as<uint32_t>());
+      if (wide) {
+        if (pad < wide_dyn_bytes<kWideWarps>()) pad = (unsigned)wide_dyn_bytes<kWideWarps>();
+        k_iterate<kWideWarps><<<(unsigned)ns, kWideWarps * 32, pad, l.stream>>>(b, l.order.as<uint32_t>());
+      } else {
+        k_iterate<2><<<(unsigned)ns, 64, pad, l.stream>>>(b, l.order.as<uint32_t>());
+      }
       CK(cudaGetLastError());
       l.toc(l.acc.ms_iterate);
       l.acc.launches++;

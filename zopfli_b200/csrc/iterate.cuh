@@ -1,6 +1,7 @@
 // k_iterate: the whole ZopfliLZ77Optimal loop for one deflate block in one persistent CTA of two
 // warps -- warp 0 runs the algorithm, warp 1 feeds the forward DP
-// (/root/reference/src/zopfli/squeeze.c:446-526; fixed-tree variant :528-560).
+// (/root/reference/src/zopfli/squeeze.c:446-526; fixed-tree variant :528-560).  The wide form (eight
+// warps, for launches that take whole SMs) runs trace-back and follow-path on all of them.
 //
 //   per iteration:  cost model constants (GetCostModelMinCost squeeze.c:163-198)
 //                   forward DP          (GetBestLengths squeeze.c:217-309)   push form, pending costs
@@ -177,6 +178,9 @@ __device__ __forceinline__ void mbar_wait_a(uint32_t bar_a, uint32_t parity) {
   } while (!done);
 }
 __device__ __forceinline__ void cta_sync64() { asm volatile("bar.sync 1, 64;" ::: "memory"); }
+// every warp of the wide form (trace-back and follow-path); cta_sync64 counts only warp 0 and the feeder
+template <int NW>
+__device__ __forceinline__ void cta_sync_all() { asm volatile("bar.sync 2, %0;" ::"n"(NW * 32) : "memory"); }
 __device__ __forceinline__ uint32_t lds_u16(uint32_t a) {
   uint32_t v;
   asm volatile("ld.shared.u16 %0, [%1];" : "=r"(v) : "r"(a) : "memory");
@@ -450,15 +454,274 @@ __device__ __forceinline__ uint32_t first_dist_of_symbol(int sd) {  // squeeze.c
   return sd < 4 ? (uint32_t)sd + 1 : 1u + ((2u + (uint32_t)(sd & 1)) << (sd / 2 - 1));
 }
 
+// FollowPath (squeeze.c:338-389) of the traced symbols psym[cursor + t], t in [t0, t1), by one warp: store
+// entries t of cl / cd, histogram into `hist`.  128 symbols in flight per trip, fetched one trip ahead.
+// The wide form's slice of the loop the two-warp form runs inline over [0, nsym) (calling this function
+// there instead changes that kernel's register allocation).
+__device__ __forceinline__ void follow_path(const Batch& b, const SegDesc& sd, const uint8_t* in, const uint32_t* psym,
+                                            uint32_t cursor, uint32_t t0, uint32_t t1, uint16_t* cl, uint16_t* cd,
+                                            uint32_t* hist, uint32_t lane) {
+  uint32_t en[4];  // symbols of the next trip, fetched one trip ahead
+#pragma unroll
+  for (int u = 0; u < 4; u++) {
+    const uint32_t t = t0 + u * 32 + lane;
+    en[u] = t < t1 ? psym[cursor + t] : 1u;  // dummy literal at position 0 for the tail
+  }
+  for (uint32_t base = t0; base < t1; base += 128) {
+    uint32_t e[4];
+    uint4 ra[4], rc[4];
+    uint32_t by[4];
+#pragma unroll
+    for (int u = 0; u < 4; u++) {
+      e[u] = en[u];
+      const uint32_t t = base + 128 + u * 32 + lane;
+      en[u] = t < t1 ? psym[cursor + t] : 1u;
+    }
+#pragma unroll
+    for (int u = 0; u < 4; u++) {
+      const uint32_t len = e[u] & 511u, pj = e[u] >> 9;
+      const uint4* r4 = (const uint4*)(b.runs + (sd.pos_off + pj) * kRunSlots);
+      if (len >= (uint32_t)kMinMatch) { ra[u] = r4[0]; rc[u] = r4[1]; by[u] = 0; }
+      else { ra[u] = make_uint4(0, 0, 0, 0); rc[u] = ra[u]; by[u] = in[pj]; }
+    }
+#pragma unroll
+    for (int u = 0; u < 4; u++) {
+      const uint32_t t = base + u * 32 + lane;
+      if (t >= t1) continue;
+      const uint32_t len = e[u] & 511u;
+      if (len >= (uint32_t)kMinMatch) {
+        const uint4 a = ra[u], c = rc[u];
+        uint32_t x = c.w;
+        if (c.w & kOverflowBit) {
+          x = 0;
+          if (len > run_len(c.z)) {
+            const uint32_t off = c.w & ~kOverflowBit, cnt = b.ovf[off];
+            for (uint32_t i = 0; i < cnt; i++) { uint32_t y = b.ovf[off + 1 + i]; if (run_len(y) >= len) { x = y; break; } }
+          }
+        }
+        if (len <= run_len(c.z)) x = c.z;
+        if (len <= run_len(c.y)) x = c.y;
+        if (len <= run_len(c.x)) x = c.x;
+        if (len <= run_len(a.w)) x = a.w;
+        if (len <= run_len(a.z)) x = a.z;
+        if (len <= run_len(a.y)) x = a.y;
+        if (len <= run_len(a.x)) x = a.x;
+        cl[t] = (uint16_t)len; cd[t] = (uint16_t)run_dist(x);
+        atomicAdd(&hist[length_symbol((int)len)], 1u);
+        atomicAdd(&hist[288 + run_dsym(x)], 1u);
+      } else {
+        cl[t] = (uint16_t)by[u]; cd[t] = 0;
+        atomicAdd(&hist[by[u]], 1u);
+      }
+    }
+  }
+}
+
+// ---- wide form of k_iterate (NW = 8 warps; launches whose CTAs take a whole SM) ----
+// The DP runs on warp 0 and the feeder exactly as in the two-warp form while warps 2.. wait at
+// cta_sync_all; trace-back and follow-path then run on every warp.  Their working set lies in the dynamic
+// shared memory the launch pads anyway, after IterDyn.
+constexpr int kWideWarps = 8;
+constexpr uint32_t kTrSegLen = 128;   // positions per speculative chain of the trace-back
+template <int NW>
+struct WideSmem {
+  static constexpr uint32_t kSeg = NW * 32, kWin = kSeg * kTrSegLen;   // one segment per thread
+  uint16_t la[kWin];                  // trace-back window: length_array slice
+  uint16_t mark[kWin];                // visit number of a node on its segment's speculative chain (0: not visited)
+  uint32_t cnt[kSeg], exit[kSeg];     // length and exit node of each segment's speculative chain
+  uint32_t in[kSeg], out[kSeg];       // the true path in each segment: entry node, exit node,
+  uint32_t ns[kSeg], off[kSeg];       //   symbols, and symbols of the segments above it in the window
+  uint32_t hist[NW][320];             // follow-path histogram of each warp
+  uint32_t idx, cursor, nact, curbuf; // next window's top node, psym cursor, live segments; warp 0's curbuf
+};
+constexpr size_t kWideOff = (sizeof(IterDyn) + 15) & ~(size_t)15;   // offset of WideSmem in the dynamic shared memory
+template <int NW>
+constexpr size_t wide_dyn_bytes() { return kWideOff + sizeof(WideSmem<NW>); }
+
+// one hop of the trace-back from node i: length_array[i] clamped to [1, i] so a corrupted chain cannot hang
+__device__ __forceinline__ uint32_t tr_hop(uint32_t la_a, uint32_t wlo, uint32_t i) {
+  uint32_t l;
+  asm volatile("ld.shared.u16 %0, [%1];" : "=r"(l) : "r"(la_a + (i - wlo) * 2));
+  return min(max(l, 1u), i);
+}
+struct TrSeg { uint32_t hi, floor_; bool live; };   // segment sg of a window: positions (floor_, hi]
+__device__ __forceinline__ TrSeg tr_seg(uint32_t idx, uint32_t wlo, uint32_t sg) {
+  const uint32_t hi = idx >= sg * kTrSegLen ? idx - sg * kTrSegLen : 0u;
+  const uint32_t lo = hi >= kTrSegLen ? hi - kTrSegLen : 0u;
+  return {hi, lo > wlo ? lo : (wlo > 0 ? wlo - 1 : 0u), hi > 0 && hi >= wlo};   // stop below the window as well
+}
+// the path entering a segment at node i: hop until it meets the segment's speculative chain at its node
+// number m (then it follows the chain's cnt - m + 1 remaining hops to ex) or leaves the segment.  Returns the
+// exit node; n = the symbols on the way.
+__device__ __forceinline__ uint32_t tr_walk(uint32_t la_a, uint32_t mk_a, uint32_t wlo, uint32_t i, uint32_t floor_,
+                                            uint32_t cnt, uint32_t ex, uint32_t& n) {
+  uint32_t h = 0;
+  while (i > floor_) {
+    uint32_t mk;
+    asm volatile("ld.shared.u16 %0, [%1];" : "=r"(mk) : "r"(mk_a + (i - wlo) * 2));
+    if (mk) { n = h + cnt - mk + 1; return ex; }
+    i -= tr_hop(la_a, wlo, i);
+    h++;
+  }
+  n = h;
+  return i;
+}
+
+// TraceBackwards (squeeze.c:317-336) on every thread of the CTA.  Same speculative scheme as the two-warp
+// form, with one 128-position segment per thread and windows of kWin positions:
+//   pass 1  every thread chases the chain from the top of its segment and numbers the nodes it visits;
+//   pass 2  every segment assumes the path enters it where the chain of the segment above leaves, and walks
+//           to where it meets its own chain (tr_walk); warp 0 then checks the assumptions 32 segments at a
+//           time (entry == exit of the segment above) and re-walks only the segments where one failed;
+//   pass 3  every segment writes its symbols at their offset in psym.
+// psym[cursor .. nb] comes out as (start position << 9 | length) of the path, in order.  Returns cursor.
+template <int NW>
+__device__ __noinline__ uint32_t wide_trace(WideSmem<NW>& W, const uint16_t* la, uint32_t* psym, uint32_t nb) {
+  constexpr uint32_t kSeg = WideSmem<NW>::kSeg, kWin = WideSmem<NW>::kWin, NT = NW * 32;
+  const uint32_t s = threadIdx.x, lane = s & 31u, full = 0xffffffffu;
+  const uint32_t la_a = smem_u32(&W.la[0]), mk_a = smem_u32(&W.mark[0]);
+  const bool la_odd = (((uintptr_t)la) >> 1) & 1;  // make 4-byte loads aligned
+  uint32_t idx = nb, cursor = nb + 1;
+  while (idx > 0) {
+    // window covers la[wlo .. idx], wlo chosen so that &la[wlo] is 4-byte aligned
+    uint32_t wlo = idx >= kWin - 8 ? idx - (kWin - 9) : 0u;
+    if (((wlo & 1u) != 0) != la_odd) wlo = wlo > 0 ? wlo - 1 : 0;
+    const uint32_t cnt = idx - wlo + 1;
+    if ((((uintptr_t)(la + wlo)) & 3) == 0) {
+      const uint32_t* src = (const uint32_t*)(la + wlo);
+      uint32_t* dst = (uint32_t*)&W.la[0];
+      const uint32_t nw = (cnt + 1) / 2;
+      for (uint32_t tb = 0; tb < nw; tb += NT * 8) {  // 8 loads in flight per thread
+        uint32_t v[8];
+#pragma unroll
+        for (int u = 0; u < 8; u++) { const uint32_t t = tb + u * NT + s; v[u] = t < nw ? src[t] : 0u; }
+#pragma unroll
+        for (int u = 0; u < 8; u++) { const uint32_t t = tb + u * NT + s; if (t < nw) dst[t] = v[u]; }
+      }
+    } else {
+      for (uint32_t t = s; t < cnt; t += NT) W.la[t] = la[wlo + t];
+    }
+    for (uint32_t t = s; t < (cnt + 7) / 8; t += NT) ((uint4*)&W.mark[0])[t] = make_uint4(0, 0, 0, 0);
+    cta_sync_all<NW>();
+    // ---- pass 1: the speculative chain of this thread's segment ----
+    const TrSeg g = tr_seg(idx, wlo, s);
+    uint32_t exit_s = g.hi, cnt_s = 0;
+    if (g.live) {
+      uint32_t i = g.hi;
+      while (i > g.floor_) {
+        cnt_s++;
+        asm volatile("st.shared.u16 [%0], %1;" ::"r"(mk_a + (i - wlo) * 2), "h"((unsigned short)cnt_s) : "memory");
+        i -= tr_hop(la_a, wlo, i);
+      }
+      exit_s = i;
+    }
+    W.cnt[s] = cnt_s;
+    W.exit[s] = exit_s;
+    cta_sync_all<NW>();
+    // ---- pass 2: walk from the assumed entry ----
+    if (g.live) {
+      const uint32_t e = s == 0 ? idx : W.exit[s - 1];
+      uint32_t n;
+      W.in[s] = e;
+      W.out[s] = tr_walk(la_a, mk_a, wlo, e, g.floor_, cnt_s, exit_s, n);
+      W.ns[s] = n;
+    }
+    cta_sync_all<NW>();
+    // ---- pass 2, warp 0: accept every segment whose entry is the exit of the one above (one ballot per 32 of
+    // them), re-walk the first one that is not from its true entry, go on behind it; stop where the path leaves
+    // the window or ends ----
+    if (s < 32) {
+      uint32_t e = idx, tot = 0, nact = kSeg;
+      for (uint32_t s0 = 0; s0 < kSeg; s0 += 32) {
+        const uint32_t sg = s0 + lane;
+        const bool dead = !tr_seg(idx, wlo, sg).live;
+        uint32_t gin = W.in[sg], gout = W.out[sg], gn = W.ns[sg];
+        uint32_t start = 0, stop = 32;  // lanes below start are settled; the path stops at lane `stop`
+        while (start < 32) {
+          const uint32_t up = __shfl_up_sync(full, gout, 1);
+          const uint32_t ent = lane == start ? e : up;   // true entry, if the lanes in between are right
+          const bool halt = dead || ent == 0 || ent < wlo;
+          const uint32_t bad = __ballot_sync(full, lane >= start && (halt || gin != ent));
+          if (bad == 0) { e = __shfl_sync(full, gout, 31); break; }
+          const uint32_t f = __ffs(bad) - 1;
+          e = __shfl_sync(full, ent, f);
+          if (__shfl_sync(full, halt ? 1u : 0u, f)) { stop = f; break; }
+          const TrSeg gf = tr_seg(idx, wlo, s0 + f);
+          uint32_t n;
+          const uint32_t o = tr_walk(la_a, mk_a, wlo, e, gf.floor_, W.cnt[s0 + f], W.exit[s0 + f], n);
+          if (lane == f) { gin = e; gout = o; gn = n; }
+          e = o;
+          start = f + 1;
+        }
+        const uint32_t v = lane < stop ? gn : 0u;
+        uint32_t incl = v;
+#pragma unroll
+        for (uint32_t d = 1; d < 32; d <<= 1) { const uint32_t o = __shfl_up_sync(full, incl, d); if (lane >= d) incl += o; }
+        if (lane < stop) { W.in[sg] = gin; W.ns[sg] = gn; W.off[sg] = tot + incl - v; }
+        tot += __shfl_sync(full, incl, 31);
+        if (stop < 32) { nact = s0 + stop; break; }
+      }
+      if (lane == 0) { W.nact = nact; W.idx = e; W.cursor = cursor - tot; }
+    }
+    cta_sync_all<NW>();
+    // ---- pass 3: write the symbols ----
+    const uint32_t nact = W.nact, nidx = W.idx, ncur = W.cursor;
+    if (s < nact) {
+      uint32_t i = W.in[s];
+      const uint32_t n = W.ns[s], top = cursor - W.off[s];
+      for (uint32_t k = 0; k < n; k++) {
+        const uint32_t l = tr_hop(la_a, wlo, i);
+        i -= l;
+        psym[top - 1 - k] = (i << 9) | l;
+      }
+    }
+    idx = nidx;
+    cursor = ncur;
+    cta_sync_all<NW>();  // the next window reuses la, mark and the segment tables
+  }
+  return cursor;
+}
+
+// follow-path + histogram on every warp: warp w takes a contiguous slice of the nsym symbols and counts into a
+// histogram of its own; warp 0 adds them up into s.hist (integer sums: exact in any order)
+template <int NW>
+__device__ __noinline__ void wide_follow(WideSmem<NW>& W, uint32_t* hist_out, const Batch& b, const SegDesc& sd,
+                                         const uint8_t* in, const uint32_t* psym, uint32_t cursor, uint32_t nsym) {
+  const uint32_t lane = threadIdx.x & 31u, wid = threadIdx.x >> 5;
+  const int cb = (int)W.curbuf;
+  uint32_t* h = W.hist[wid];
+  for (int i = lane; i < 320; i += 32) h[i] = 0;
+  __syncwarp();
+  const uint32_t per = ((nsym + NW - 1) / NW + 31) & ~31u;
+  const uint32_t t0 = min(nsym, wid * per), t1 = min(nsym, t0 + per);
+  follow_path(b, sd, in, psym, cursor, t0, t1, b.st_ll[cb] + sd.pos_off, b.st_d[cb] + sd.pos_off, h, lane);
+  cta_sync_all<NW>();
+  if (wid == 0) {
+    for (int i = lane; i < 320; i += 32) {
+      uint32_t c = 0;
+#pragma unroll
+      for (int w = 0; w < NW; w++) c += W.hist[w][i];
+      hist_out[i] = c;
+    }
+    __syncwarp();
+  }
+}
+
 // Two warps per block.  Warp 0 runs the whole algorithm; warp 1 is the FEEDER of the forward DP: it
 // issues the TMA copies of the match-table rows, stages the per-position scalars (literal cost,
 // match length, general-path flags) and writes the finished length_array entries back to global
 // memory, three groups of 32 positions ahead of / behind the DP warp (full[] / empty[] mbarriers).
 // Outside the DP phase it is parked at a named barrier.
-__global__ void __launch_bounds__(64, 4) k_iterate(Batch b, const uint32_t* __restrict__ order) {
+// NW = 2: that pair alone, four CTAs per SM.  NW = 8 (wide form, launches that take whole SMs): warps 2..7
+// wait at cta_sync_all during the DP; trace-back and follow-path run on all eight warps (wide_trace,
+// wide_follow), the feeder included.
+template <int NW>
+__global__ void __launch_bounds__(NW * 32, NW == 2 ? 4 : 1) k_iterate(Batch b, const uint32_t* __restrict__ order) {
+  static_assert(NW == 2 || NW == 8, "k_iterate: two warps, or the wide form");
   __shared__ IterSmem s;
   extern __shared__ __align__(16) unsigned char zb_iter_dyn[];
   IterDyn& dyn = *reinterpret_cast<IterDyn*>(zb_iter_dyn);
+  WideSmem<NW>& W = *reinterpret_cast<WideSmem<NW>*>(zb_iter_dyn + kWideOff);   // wide form only
   const uint32_t seg = order[blockIdx.x], lane = threadIdx.x & 31u, wid = threadIdx.x >> 5;
   const SegDesc sd = b.segs[seg];
   if (sd.mode == 0) return;
@@ -485,7 +748,7 @@ __global__ void __launch_bounds__(64, 4) k_iterate(Batch b, const uint32_t* __re
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   // the staged distance symbols index the cost table: keep every byte of the staging area <= 30
-  for (uint32_t t = threadIdx.x; t < sizeof(s.u.dp.dsx) / 4; t += 64) ((uint32_t*)&s.u.dp.dsx[0])[t] = 0;
+  for (uint32_t t = threadIdx.x; t < sizeof(s.u.dp.dsx) / 4; t += NW * 32) ((uint32_t*)&s.u.dp.dsx[0])[t] = 0;
   __syncthreads();
   uint32_t seq_base = 0;  // running group sequence number: stage = seq & 3, parity = (seq >> 2) & 1
   uint32_t igroups = 0;   // groups that ran in the integer window
@@ -493,6 +756,18 @@ __global__ void __launch_bounds__(64, 4) k_iterate(Batch b, const uint32_t* __re
   uint32_t i_gen = 0;     // generation of the integer tables (DP warp); a stage is usable only if its tag equals it
   const uint32_t ngroups = (nb + 31) >> 5;
 
+  if constexpr (NW > 2) {
+    if (wid >= 2) {
+      // ================================================================== helper warps (wide form)
+      for (;;) {
+        cta_sync_all<NW>();  // (C) the DP is over and length_array complete, or warp 0 has finished
+        if (*(volatile uint32_t*)&s.go == 0) break;
+        const uint32_t cursor = wide_trace<NW>(W, la, psym, nb);
+        wide_follow<NW>(W, s.hist, b, sd, in, psym, cursor, nb + 1 - cursor);
+      }
+      return;
+    }
+  }
   if (wid == 1) {
     // ================================================================== feeder warp
     for (;;) {
@@ -546,7 +821,13 @@ __global__ void __launch_bounds__(64, 4) k_iterate(Batch b, const uint32_t* __re
       }
       seq_base = end;
       cta_sync64();  // (B) length_array complete
+      if constexpr (NW > 2) {
+        cta_sync_all<NW>();  // (C)
+        const uint32_t cursor = wide_trace<NW>(W, la, psym, nb);
+        wide_follow<NW>(W, s.hist, b, sd, in, psym, cursor, nb + 1 - cursor);
+      }
     }
+    if constexpr (NW > 2) cta_sync_all<NW>();  // (C) at warp 0's exit: releases the helper warps
     return;
   }
   // ====================================================================== DP warp (warp 0)
@@ -1213,7 +1494,11 @@ __global__ void __launch_bounds__(64, 4) k_iterate(Batch b, const uint32_t* __re
     // third pass re-walks the chains 32 wide and writes the adopted nodes.  Each symbol is emitted
     // as (start position << 9 | length); psym[cursor .. nb+1) holds the symbols in order.
     uint32_t cursor = nb + 1;
-    {
+    if constexpr (NW > 2) {
+      if (lane == 0) W.curbuf = (uint32_t)curbuf;
+      cta_sync_all<NW>();  // (C) every warp joins for trace-back and follow-path
+      cursor = wide_trace<NW>(W, la, psym, nb);
+    } else {
       uint32_t idx = nb;  // current true path node
       const uint32_t la_a = smem_u32(&s.u.tr.la[0]), mk_a = smem_u32(&s.u.tr.mark[0]);
       const bool la_odd = (((uintptr_t)la) >> 1) & 1;  // make 4-byte loads aligned
@@ -1307,6 +1592,9 @@ __global__ void __launch_bounds__(64, 4) k_iterate(Batch b, const uint32_t* __re
     ZB_TICK(2);
 
     // ------------------------------------------------------------------ follow path + histogram
+    if constexpr (NW > 2) {
+      wide_follow<NW>(W, s.hist, b, sd, in, psym, cursor, nsym);
+    } else {
     uint16_t* cl = b.st_ll[curbuf] + sd.pos_off;
     uint16_t* cd = b.st_d[curbuf] + sd.pos_off;
     for (int i = lane; i < 320; i += 32) s.hist[i] = 0;
@@ -1366,6 +1654,7 @@ __global__ void __launch_bounds__(64, 4) k_iterate(Batch b, const uint32_t* __re
       }
     }
     __syncwarp();
+    }
     ZB_TICK(3);
     if (fixed) { bestbuf = curbuf; best_size = nsym; bestcost = 0; it++; break; }
     if (lane == 0) s.hist[256] = 1;  // deflate.c:575 and squeeze.c:409
@@ -1429,6 +1718,7 @@ __global__ void __launch_bounds__(64, 4) k_iterate(Batch b, const uint32_t* __re
   if (lane == 0) s.go = 0;
   __syncwarp();
   cta_sync64();  // (A) releases the feeder warp for good
+  if constexpr (NW > 2) cta_sync_all<NW>();  // (C) with go == 0: releases the helper warps; the feeder joins after (A)
   if (lane == 0) {
     for (int i = 0; i < 6; i++) js->cyc[i] = (uint64_t)cyc[i];
     js->best_size = best_size;
