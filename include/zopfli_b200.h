@@ -104,6 +104,28 @@ void ZopfliB200CompressDevice(const ZopfliOptions* options, ZopfliFormat output_
                               const unsigned char* in, size_t insize, const unsigned char* dev_in,
                               unsigned char** out, size_t* outsize);
 
+/* ---- input and output in device memory ----
+ * ZopfliCompress (zopfli.h:86-88) of the insize bytes at device address dev_in, result in device memory.
+ * The bytes of *dev_out equal what ZopfliCompress(options, output_type, <same bytes>) returns.
+ * dev_in: any alignment, nothing past insize is read; work is ordered after what is queued on cuda_stream
+ * (a cudaStream_t of dev_in's device, NULL = legacy default stream), and cuda_stream is made to wait for the
+ * result.  Runs on the device that owns dev_in (one GPU: ZOPFLI_B200_GPUS does not apply); the call blocks
+ * until the result is complete.  The CRC-32 / Adler-32 of the trailer is computed on the device, so no byte of
+ * the input or of the stream crosses PCIe.  *dev_out: exactly *outsize bytes from cudaMallocAsync on
+ * cuda_stream; the caller owns it (cudaFreeAsync / cudaFree / ZopfliB200FreeDevice).  Unlike ZopfliCompress
+ * nothing is appended: *dev_out and *outsize are outputs only.  With insize == 0, dev_in may be NULL and the
+ * call runs on the current device.  Updates ZopfliB200LastMasterBitOffsets and prints the verbose reports
+ * as ZopfliCompress does.  Returns 0, or nonzero with the outputs untouched when dev_in is not device memory,
+ * an output pointer is NULL or the format is unknown. */
+int ZopfliB200CompressDeviceToDevice(const ZopfliOptions* options, ZopfliFormat output_type,
+                                     const unsigned char* dev_in, size_t insize, void* cuda_stream,
+                                     unsigned char** dev_out, size_t* outsize);
+void ZopfliB200FreeDevice(void* dev_ptr, void* cuda_stream); /* cudaFreeAsync on the device that owns dev_ptr */
+/* zlib-compatible CRC-32 / Adler-32 of device bytes (any alignment, size 0 with NULL allowed), computed on
+ * the device; blocking, ordered after cuda_stream.  Return nonzero when dev_in is not device memory. */
+int ZopfliB200Crc32Device(const unsigned char* dev_in, size_t size, void* cuda_stream, uint32_t* crc);
+int ZopfliB200Adler32Device(const unsigned char* dev_in, size_t size, void* cuda_stream, uint32_t* adler);
+
 /* ---- several GPUs, one stream (SURVEY 8(e)) ----
  * The master blocks of one input (the reference's independent unit, deflate.c:908-931) are sharded
  * over the GPUs of one box; NCCL scatters the byte ranges (+ 32 KiB dictionary) from rank 0's GPU and
@@ -136,6 +158,9 @@ uint32_t ZopfliB200Crc32(const unsigned char* data, size_t size);
 uint32_t ZopfliB200Crc32Combine(uint32_t crc1, uint32_t crc2, uint64_t len2);
 /* Adler-32 of the zlib trailer (zlib_container.c:29-48), threaded with an exact combination. */
 uint32_t ZopfliB200Adler32(const unsigned char* data, size_t size);
+/* The slice algebra of the device checksums (csrc/checksum.hpp) run on the host: the input cut into
+ * slices of slice_bytes, each reduced on its own and combined.  kind 0: CRC-32, 1: Adler-32. */
+uint32_t ZopfliB200HostChecksumSliced(const unsigned char* data, size_t size, size_t slice_bytes, int kind);
 
 /* Engine control / introspection. */
 typedef struct ZopfliB200Stats {

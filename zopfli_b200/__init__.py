@@ -54,7 +54,8 @@ EXPORTS = ["ZopfliInitOptions", "ZopfliCompress", "ZopfliDeflate", "ZopfliDeflat
            "ZopfliB200DeflateSpan", "ZopfliB200AppendSpan", "ZopfliB200LastMasterBitOffsets", "ZopfliB200Crc32", "ZopfliB200Crc32Combine", "ZopfliB200Adler32", "ZopfliB200CompressDevice",
            "ZopfliB200DistUniqueId", "ZopfliB200DistInit", "ZopfliB200DistCompress", "ZopfliB200DistFinalize", "ZopfliB200DistShard", "ZopfliB200DistPlacement",
            "ZopfliB200GetStats", "ZopfliB200ResetStats", "ZopfliB200SetStream", "ZopfliB200Device",
-           "ZopfliB200Version"]
+           "ZopfliB200Version", "ZopfliB200CompressDeviceToDevice", "ZopfliB200FreeDevice", "ZopfliB200Crc32Device",
+           "ZopfliB200Adler32Device", "ZopfliB200HostChecksumSliced"]
 
 
 def _pad(data):
@@ -86,6 +87,52 @@ class OutBuffer:
         self._ptr = None
 
     __del__ = close
+
+
+class DeviceOutBuffer:
+    """The device twin of OutBuffer: the cudaMallocAsync()ed result of ZopfliB200CompressDeviceToDevice,
+    owned by this object.  Exposes __cuda_array_interface__ (1-D uint8) so torch.as_tensor() wraps it
+    without a copy; freed with ZopfliB200FreeDevice on the call's stream on close() / garbage collection."""
+
+    def __init__(self, lib, ptr, size, stream):
+        self._lib, self._ptr, self.size, self._stream = lib, ptr, size, stream
+
+    def __len__(self):
+        return self.size
+
+    @property
+    def ptr(self) -> int:
+        return (self._ptr.value or 0) if self._ptr is not None else 0
+
+    @property
+    def __cuda_array_interface__(self):
+        if self._ptr is None:
+            raise ValueError("DeviceOutBuffer is closed")
+        return {"shape": (self.size,), "typestr": "|u1", "data": (self.ptr, False), "version": 2}
+
+    def close(self):
+        if self._ptr is not None and self._ptr.value:
+            self._lib.ZopfliB200FreeDevice(self._ptr, self._stream)
+        self._ptr = None
+
+    __del__ = close
+
+
+def _torch_stream(t, stream):
+    """the cudaStream_t handle of `stream` (a torch.cuda.Stream, a raw handle, or None = t's current stream)"""
+    import torch
+    if stream is None:
+        stream = torch.cuda.current_stream(t.device)
+    return stream.cuda_stream if hasattr(stream, "cuda_stream") else int(stream)
+
+
+def _device_bytes(t):
+    """(address, nbytes) of the raw bytes of a contiguous CUDA tensor"""
+    if not t.is_cuda:
+        raise ValueError("expected a CUDA tensor")
+    if not t.is_contiguous():
+        raise ValueError("expected a contiguous tensor (its bytes are compressed as laid out; copy it first)")
+    return t.data_ptr(), t.numel() * t.element_size()
 
 
 class Library:
@@ -141,6 +188,17 @@ class Library:
         L.ZopfliB200Crc32Combine.restype = C.c_uint32
         L.ZopfliB200Adler32.argtypes = [vp, sz]
         L.ZopfliB200Adler32.restype = C.c_uint32
+        L.ZopfliB200HostChecksumSliced.argtypes = [vp, sz, sz, C.c_int]
+        L.ZopfliB200HostChecksumSliced.restype = C.c_uint32
+        # device-resident calls (csrc/device_api.cpp); a host-only test build of the ABI does not export them
+        for name, args, res in (("ZopfliB200CompressDeviceToDevice",
+                                 [C.POINTER(ZopfliOptions), C.c_int, vp, sz, vp, C.POINTER(vp), C.POINTER(sz)], C.c_int),
+                                ("ZopfliB200FreeDevice", [vp, vp], None),
+                                ("ZopfliB200Crc32Device", [vp, sz, vp, C.POINTER(C.c_uint32)], C.c_int),
+                                ("ZopfliB200Adler32Device", [vp, sz, vp, C.POINTER(C.c_uint32)], C.c_int)):
+            f = getattr(L, name, None)
+            if f is not None:
+                f.argtypes, f.restype = args, res
         L.ZopfliB200DistUniqueId.argtypes = [vp]
         L.ZopfliB200DistInit.argtypes = [C.c_int, C.c_int, vp]
         L.ZopfliB200DistCompress.argtypes = [C.POINTER(ZopfliOptions), C.c_int, vp, sz, C.c_int, C.POINTER(vp), C.POINTER(sz)]
@@ -340,6 +398,45 @@ class Library:
 
     def crc32_combine(self, crc1, crc2, len2) -> int:
         return int(self.lib.ZopfliB200Crc32Combine(crc1, crc2, len2))
+
+    def host_checksum_sliced(self, data: bytes, slice_bytes: int, kind: int) -> int:
+        """the device checksums' slice algebra on the host; kind 0 CRC-32, 1 Adler-32"""
+        a = _pad(data)
+        return int(self.lib.ZopfliB200HostChecksumSliced(a.ctypes.data, len(data), slice_bytes, kind))
+
+    # ---- input and output in device memory (ZopfliB200CompressDeviceToDevice) ----
+    def compress_device_ptr(self, dev_ptr, nbytes, fmt=ZOPFLI_FORMAT_GZIP, stream=0, **kw) -> DeviceOutBuffer:
+        """ZopfliCompress of nbytes at device address dev_ptr (any alignment); the result stays on the device.
+        stream: cudaStream_t handle the call is ordered after (0 = legacy default stream)."""
+        o = self.options(**kw)
+        out, n = C.c_void_p(None), C.c_size_t(0)
+        if self.lib.ZopfliB200CompressDeviceToDevice(C.byref(o), fmt, dev_ptr, nbytes, stream, C.byref(out), C.byref(n)) != 0:
+            raise ValueError("ZopfliB200CompressDeviceToDevice: the input is not device memory, or the format is unknown")
+        return DeviceOutBuffer(self.lib, out, n.value, stream)
+
+    def compress_device(self, t, fmt=ZOPFLI_FORMAT_GZIP, stream=None, **kw):
+        """ZopfliCompress of the raw bytes of a contiguous CUDA tensor -> uint8 tensor on the same device that
+        wraps the library's allocation (no copy).  Ordered after `stream` (default: t's current stream), which
+        is made to wait for the result."""
+        import torch
+        ptr, nbytes = _device_bytes(t)
+        buf = self.compress_device_ptr(ptr, nbytes, fmt, _torch_stream(t, stream), **kw)
+        return torch.as_tensor(buf)  # keeps buf alive as long as the tensor lives
+
+    def _device_checksum(self, fn, t, stream):
+        ptr, nbytes = _device_bytes(t)
+        v = C.c_uint32(0)
+        if fn(ptr, nbytes, _torch_stream(t, stream), C.byref(v)) != 0:
+            raise ValueError("not device memory")
+        return int(v.value)
+
+    def crc32_device(self, t, stream=None) -> int:
+        """zlib.crc32 of the raw bytes of a contiguous CUDA tensor, computed on its device"""
+        return self._device_checksum(self.lib.ZopfliB200Crc32Device, t, stream)
+
+    def adler32_device(self, t, stream=None) -> int:
+        """zlib.adler32 of the raw bytes of a contiguous CUDA tensor, computed on its device"""
+        return self._device_checksum(self.lib.ZopfliB200Adler32Device, t, stream)
 
     def splice_spans(self, spans, prefix=b"", bp0=0) -> tuple[bytes, int]:
         """appends spans behind `prefix`, whose last byte has bp0 bits in use -> (bytes, final bp)"""

@@ -1,6 +1,7 @@
 // C-ABI of libzopfli.so.1 (zopfli-b200): the reference's public entry points
 // (/root/reference/src/zopfli/zopfli.h, deflate.h, gzip_container.h, zlib_container.h) plus the
-// seams declared in include/zopfli_b200.h.
+// seams declared in include/zopfli_b200.h.  The calls whose input and result live in device memory are
+// in device_api.cpp.
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -12,7 +13,9 @@
 #include <vector>
 
 #include "../../include/zopfli_b200.h"
+#include "api.hpp"
 #include "batched_split.hpp"
+#include "checksum.hpp"
 #include "dist.hpp"
 #include "dist_layout.hpp"
 #include "driver.hpp"
@@ -32,15 +35,44 @@ std::mutex g_api_mu;   // guards g_total_ms and g_last_layout
 double g_total_ms = 0;
 std::vector<uint64_t> g_last_layout;  // bit offset of every unit (master block) of the most recent deflate call
 
+}  // namespace
+
+namespace zb {
+
+double api_now_ms() { return now_ms(); }
+
+void api_call_done(std::vector<uint64_t>& layout, double t0) {
+  std::lock_guard<std::mutex> g(g_api_mu);
+  g_last_layout.swap(layout);
+  g_total_ms += now_ms() - t0;
+}
+
+// header bytes of the gzip (gzip_container.c:95-104) or zlib (zlib_container.c:58-64) container; 0 for raw deflate
+int container_header(ZopfliFormat fmt, unsigned char* hdr) {
+  if (fmt == ZOPFLI_FORMAT_GZIP) {
+    static const unsigned char gz[10] = {31, 139, 8, 0, 0, 0, 0, 0, 2, 3};
+    memcpy(hdr, gz, 10);
+    return 10;
+  }
+  if (fmt == ZOPFLI_FORMAT_ZLIB) {
+    unsigned cmfflg = 256 * 120 + 3 * 64;
+    cmfflg += 31 - cmfflg % 31;
+    hdr[0] = (unsigned char)(cmfflg / 256);
+    hdr[1] = (unsigned char)(cmfflg % 256);
+    return 2;
+  }
+  return 0;
+}
+
+}  // namespace zb
+
+namespace {
+
 // ---- CRC-32 (gzip_container.c:27-81 computes the same polynomial bytewise): slicing-by-8 ----
 uint32_t g_crc_tab[8][256];
 std::once_flag g_crc_once;
 void crc_fill() {
-  for (uint32_t i = 0; i < 256; i++) {
-    uint32_t c = i;
-    for (int k = 0; k < 8; k++) c = (c & 1) ? 0xEDB88320u ^ (c >> 1) : c >> 1;
-    g_crc_tab[0][i] = c;
-  }
+  for (uint32_t i = 0; i < 256; i++) g_crc_tab[0][i] = crc_table_entry(0, i);
   for (uint32_t i = 0; i < 256; i++)
     for (int t = 1; t < 8; t++) g_crc_tab[t][i] = (g_crc_tab[t - 1][i] >> 8) ^ g_crc_tab[0][g_crc_tab[t - 1][i] & 255];
 }
@@ -59,35 +91,6 @@ uint32_t crc32_range(const unsigned char* p, size_t n, uint32_t crc) {  // crc i
   }
   while (n--) crc = g_crc_tab[0][(crc ^ *p++) & 255] ^ (crc >> 8);
   return crc;
-}
-// GF(2) combination of CRCs of adjacent chunks (the zlib crc32_combine construction)
-uint32_t gf2_times(const uint32_t* mat, uint32_t vec) {
-  uint32_t sum = 0;
-  for (int i = 0; vec; vec >>= 1, i++)
-    if (vec & 1) sum ^= mat[i];
-  return sum;
-}
-void gf2_square(uint32_t* sq, const uint32_t* mat) {
-  for (int n = 0; n < 32; n++) sq[n] = gf2_times(mat, mat[n]);
-}
-uint32_t crc32_combine(uint32_t crc1, uint32_t crc2, uint64_t len2) {
-  if (len2 == 0) return crc1;
-  uint32_t even[32], odd[32];
-  odd[0] = 0xEDB88320u;
-  uint32_t row = 1;
-  for (int n = 1; n < 32; n++) { odd[n] = row; row <<= 1; }
-  gf2_square(even, odd);
-  gf2_square(odd, even);
-  do {
-    gf2_square(even, odd);
-    if (len2 & 1) crc1 = gf2_times(even, crc1);
-    len2 >>= 1;
-    if (len2 == 0) break;
-    gf2_square(odd, even);
-    if (len2 & 1) crc1 = gf2_times(odd, crc1);
-    len2 >>= 1;
-  } while (len2 != 0);
-  return crc1 ^ crc2;
 }
 uint32_t crc32_parallel(const unsigned char* p, size_t n) {
   crc_init();
@@ -114,24 +117,8 @@ uint32_t crc32_parallel(const unsigned char* p, size_t n) {
 
 // ---- Adler-32 (zlib_container.c:29-48 computes it serially) ----
 // s1 = 1 + sum(d_i), s2 = sum over i of s1 after byte i (both mod 65521).  Sums of byte values and of
-// position-weighted byte values are associative, so chunks are summed in 64-bit integers by threads and
-// combined: s2(A|B) = s2(A) + len(B) * (s1(A) - 1 ... ) -- written out in adler_combine below.
-struct AdlerPart { uint64_t s1, s2, len; };  // s1 = sum of bytes, s2 = sum of (len - i) * d_i, both mod 65521
-AdlerPart adler_chunk(const unsigned char* p, size_t n) {
-  // 5552 bytes is the largest run whose 32-bit running sums cannot overflow (the zlib bound the
-  // reference also relies on with 5550)
-  uint32_t a = 0, b = 0;
-  size_t left = n;
-  while (left) {
-    const size_t k = left > 5552 ? 5552 : left;
-    for (size_t i = 0; i < k; i++) { a += p[i]; b += a; }
-    a %= 65521;
-    b %= 65521;
-    p += k;
-    left -= k;
-  }
-  return {a, b, n};
-}
+// position-weighted byte values are associative, so chunks (adler_chunk, checksum.hpp) are summed by
+// threads and combined below.
 uint32_t adler32(const unsigned char* data, size_t size) {
   unsigned nt = std::thread::hardware_concurrency();
   if (nt < 1) nt = 1;
@@ -158,8 +145,6 @@ uint32_t adler32(const unsigned char* data, size_t size) {
   return (uint32_t)((s2 << 16) | s1);
 }
 
-void put_byte(unsigned char v, unsigned char** out, size_t* outsize) { append_bytes(&v, 1, out, outsize); }
-
 std::vector<std::pair<size_t, size_t>> master_units(size_t insize, size_t mb_begin, size_t mb_end) {
   std::vector<std::pair<size_t, size_t>> u;
   for (size_t m = mb_begin; m < mb_end; m++) {
@@ -172,6 +157,14 @@ std::vector<std::pair<size_t, size_t>> master_units(size_t insize, size_t mb_beg
 size_t num_master_blocks(size_t insize) {  // deflate.c:912-924 do/while
   return insize == 0 ? 1 : (insize + kMasterBlock - 1) / kMasterBlock;
 }
+
+}  // namespace
+
+std::vector<std::pair<size_t, size_t>> zb::api_master_units(size_t insize) {
+  return master_units(insize, 0, num_master_blocks(insize));
+}
+
+namespace {
 
 bool api_debug() {
   static int v = [] { const char* e = getenv("ZOPFLI_B200_DEBUG"); return e && atoi(e) ? 1 : 0; }();
@@ -225,11 +218,11 @@ template <typename Body>
 void container_impl(const ZopfliOptions* options, ZopfliFormat fmt, const unsigned char* in, size_t insize,
                     unsigned char** out, size_t* outsize, Body body) {
   unsigned char bp = 0;
+  unsigned char hdr[10];
   if (fmt == ZOPFLI_FORMAT_GZIP) {  // gzip_container.c:84-124
     uint32_t crc = 0;
     std::thread crc_thread([&] { crc = crc32_parallel(in, insize); });  // overlaps the GPU work
-    static const unsigned char hdr[10] = {31, 139, 8, 0, 0, 0, 0, 0, 2, 3};
-    append_bytes(hdr, 10, out, outsize);
+    append_bytes(hdr, container_header(fmt, hdr), out, outsize);
     body(&bp);
     const double tj = now_ms();
     crc_thread.join();
@@ -245,10 +238,7 @@ void container_impl(const ZopfliOptions* options, ZopfliFormat fmt, const unsign
   } else if (fmt == ZOPFLI_FORMAT_ZLIB) {  // zlib_container.c:50-79
     uint32_t checksum = 0;
     std::thread adler_thread([&] { checksum = adler32(in, insize); });  // overlaps the GPU work
-    unsigned cmfflg = 256 * 120 + 3 * 64;
-    cmfflg += 31 - cmfflg % 31;
-    put_byte((unsigned char)(cmfflg / 256), out, outsize);
-    put_byte((unsigned char)(cmfflg % 256), out, outsize);
+    append_bytes(hdr, container_header(fmt, hdr), out, outsize);
     body(&bp);
     adler_thread.join();
     unsigned char tr[4] = {(unsigned char)((checksum >> 24) & 255), (unsigned char)((checksum >> 16) & 255),
@@ -393,6 +383,9 @@ int ZopfliB200DeflateSpan(const ZopfliOptions* options, const unsigned char* in,
 uint32_t ZopfliB200Crc32(const unsigned char* data, size_t size) { return crc32_parallel(data, size); }
 uint32_t ZopfliB200Crc32Combine(uint32_t crc1, uint32_t crc2, uint64_t len2) { return crc32_combine(crc1, crc2, len2); }
 uint32_t ZopfliB200Adler32(const unsigned char* data, size_t size) { return adler32(data, size); }
+uint32_t ZopfliB200HostChecksumSliced(const unsigned char* data, size_t size, size_t slice_bytes, int kind) {
+  return checksum_sliced(data, size, slice_bytes, kind);
+}
 
 int ZopfliB200AppendSpan(const unsigned char* span, size_t spansize, unsigned char* bp, unsigned char** out,
                          size_t* outsize) {

@@ -549,10 +549,8 @@ uint64_t layout_pieces(const std::vector<Piece>& pieces, size_t in_base, uint64_
   return pos;
 }
 
-void assemble(Engine& eng, const std::vector<Piece>& pieces, size_t in_base, unsigned char* bp, unsigned char** out,
-              size_t* outsize, std::vector<uint64_t>* unit_bits, bool verbose) {
-  const unsigned phase = (*outsize > 0) ? (*bp & 7u) : 0u;  // bits in use in the last byte (deflate.h:50-53)
-  std::vector<Engine::EmitPiece> ep;
+uint64_t place_pieces(const std::vector<Piece>& pieces, size_t in_base, unsigned phase, std::vector<Engine::EmitPiece>& ep,
+                      std::vector<uint64_t>* unit_bits, bool verbose) {
   const uint64_t total = layout_pieces(pieces, in_base, phase, ep, unit_bits);
   if (verbose) {  // AddLZ77Block's reports (deflate.c:718-744): growth of *outsize (= bytes touched so far) per part
     for (size_t i = 0; i < pieces.size(); i++) {
@@ -564,6 +562,14 @@ void assemble(Engine& eng, const std::vector<Piece>& pieces, size_t in_base, uns
       fprintf(stderr, "compressed block size: %d (%dk) (unc: %d)\n", (int)grown, (int)(grown / 1024), (int)(p.inend - p.instart));
     }
   }
+  return total;
+}
+
+void assemble(Engine& eng, const std::vector<Piece>& pieces, size_t in_base, unsigned char* bp, unsigned char** out,
+              size_t* outsize, std::vector<uint64_t>* unit_bits, bool verbose) {
+  const unsigned phase = (*outsize > 0) ? (*bp & 7u) : 0u;  // bits in use in the last byte (deflate.h:50-53)
+  std::vector<Engine::EmitPiece> ep;
+  const uint64_t total = place_pieces(pieces, in_base, phase, ep, unit_bits, verbose);
   const size_t nbytes = (size_t)((total + 7) / 8);
   if (nbytes == 0) return;
   unsigned char keep = 0;

@@ -55,6 +55,10 @@ void deflate_units(Engine& eng, const ZopfliOptions* opt, int btype, bool final_
 void assemble(Engine& eng, const std::vector<Piece>& pieces, size_t in_base, unsigned char* bp, unsigned char** out,
               size_t* outsize, std::vector<uint64_t>* unit_bits = nullptr, bool verbose = false);
 
+// assemble() up to the emission: layout_pieces from bit `phase`, plus the per-block verbose report
+uint64_t place_pieces(const std::vector<Piece>& pieces, size_t in_base, unsigned phase, std::vector<Engine::EmitPiece>& ep,
+                      std::vector<uint64_t>* unit_bits, bool verbose);
+
 // bit position of every piece when the first one starts at bit0; returns the end position
 uint64_t layout_pieces(const std::vector<Piece>& pieces, size_t in_base, uint64_t bit0, std::vector<Engine::EmitPiece>& ep,
                        std::vector<uint64_t>* unit_bits);

@@ -14,6 +14,7 @@
 #include <mutex>
 #include <thread>
 
+#include "checksum.cuh"
 #include "iterate.cuh"
 #include "kernels.cuh"
 #include "split.cuh"
@@ -292,6 +293,12 @@ struct Engine::Impl {
   size_t slab_idx = 0, slab_used = 0;
   DevBuf outbuf, emit_desc, err_flag;
   Stager stager;
+  // device-resident calls: the caller's stream is ordered against lane 0 through events; the checksum of
+  // the input runs on a low-priority stream of its own, beside the parse
+  cudaStream_t ck_stream = nullptr;
+  cudaEvent_t ev_user, ev_lane0, ev_ck;
+  DevBuf ck_acc;
+  int sm_count = 0;
 
   void begin_call() {  // a new input: plans of the previous call are dead
     std::lock_guard<std::mutex> g(fin_mu);
@@ -345,6 +352,12 @@ struct Engine::Impl {
     DevBuf* shared[] = {&in_buf, &same_buf, &tile_first, &next_tile, &sym_ll[0], &sym_ll[1], &sym_ll[2], &sym_d[0],
                         &sym_d[1], &sym_d[2], &outbuf, &emit_desc, &err_flag};
     for (DevBuf* d : shared) d->st = lane[0].stream;
+    int lo = 0, hi = 0;
+    CK(cudaDeviceGetStreamPriorityRange(&lo, &hi));
+    CK(cudaStreamCreateWithPriority(&ck_stream, cudaStreamNonBlocking, lo));
+    for (cudaEvent_t* e : {&ev_user, &ev_lane0, &ev_ck}) CK(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
+    ck_acc.st = ck_stream;
+    CK(cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev));
     CK(cudaFuncSetAttribute(k_match, cudaFuncAttributeMaxDynamicSharedMemorySize, kMatchSmemBytes));
     for (const void* k : {(const void*)k_iterate<2>, (const void*)k_iterate<kWideWarps>}) {
       cudaFuncAttributes fa;
@@ -374,6 +387,28 @@ struct Engine::Impl {
     CK(cudaGetLastError());
     l.toc(st_acc.ms_same);
     st_acc.launches += 3;
+  }
+
+  // zeroes the accumulator and queues the checksum (ChecksumKind) of d[0, n) on ck_stream; caller holds mu
+  void launch_checksum(const uint8_t* d, uint64_t n, int kind) {
+    ck_acc.ensure(sizeof(ChecksumAcc));
+    CK(cudaMemsetAsync(ck_acc.p, 0, sizeof(ChecksumAcc), ck_stream));
+    if (n == 0) return;
+    const void* k = kind == kCkCrc32 ? (const void*)k_crc32 : (const void*)k_adler32;
+    int per_sm = 0;
+    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k, kCkThreads, 0));
+    const uint64_t warps_wanted = n / kCkTile + 1;
+    const unsigned grid = (unsigned)std::min<uint64_t>((warps_wanted + kCkThreads / 32 - 1) / (kCkThreads / 32),
+                                                       (uint64_t)sm_count * std::max(per_sm, 1));
+    CkArgs a{d, n, ck_acc.as<ChecksumAcc>(), crc_tab()};
+    if (kind == kCkCrc32) k_crc32<<<grid, kCkThreads, 0, ck_stream>>>(a);
+    else k_adler32<<<grid, kCkThreads, 0, ck_stream>>>(a);
+    CK(cudaGetLastError());
+    st_acc.launches++;
+  }
+  static const CrcShiftTable& crc_tab() {
+    static const CrcShiftTable t = crc_shift_table();
+    return t;
   }
 
   struct Layout {
@@ -686,6 +721,65 @@ void Engine::set_input_device(const uint8_t* dev_in, size_t insize) {
   m.compute_same();
   m.lane[0].sync();
   m.begin_call();
+}
+
+void Engine::set_input_device_copy(const uint8_t* dev_src, size_t insize, void* user_stream, int checksum) {
+  std::lock_guard<std::mutex> g(p_->mu);
+  Impl& m = *p_;
+  Lane& l = m.lane[0];
+  CK(cudaSetDevice(m.dev));
+  m.in_buf.ensure(insize + 64);
+  // the lanes are non-blocking streams: they order against the caller's stream only through an event
+  CK(cudaEventRecord(m.ev_user, (cudaStream_t)user_stream));
+  CK(cudaStreamWaitEvent(l.stream, m.ev_user, 0));
+  if (insize) CK(cudaMemcpyAsync(m.in_buf.p, dev_src, insize, cudaMemcpyDeviceToDevice, l.stream));
+  CK(cudaMemsetAsync((uint8_t*)m.in_buf.p + insize, 0, 64, l.stream));
+  m.d_in = m.in_buf.as<uint8_t>();
+  m.insize = insize;
+  if (checksum != kCkNone) {
+    CK(cudaEventRecord(m.ev_lane0, l.stream));
+    CK(cudaStreamWaitEvent(m.ck_stream, m.ev_lane0, 0));
+    m.launch_checksum(m.d_in, insize, checksum);
+    CK(cudaEventRecord(m.ev_ck, m.ck_stream));
+  }
+  m.compute_same();
+  l.sync();
+  m.begin_call();
+}
+
+uint32_t Engine::checksum_device(const uint8_t* dev_in, size_t n, void* user_stream, int checksum) {
+  std::lock_guard<std::mutex> g(p_->mu);
+  Impl& m = *p_;
+  CK(cudaSetDevice(m.dev));
+  CK(cudaEventRecord(m.ev_user, (cudaStream_t)user_stream));
+  CK(cudaStreamWaitEvent(m.ck_stream, m.ev_user, 0));
+  m.launch_checksum(dev_in, n, checksum);
+  ChecksumAcc h;
+  CK(cudaMemcpyAsync(&h, m.ck_acc.p, sizeof(h), cudaMemcpyDeviceToHost, m.ck_stream));
+  CK(cudaStreamSynchronize(m.ck_stream));
+  return checksum == kCkCrc32 ? crc_finish(h.crc0, n, Impl::crc_tab()) : adler_finish(h.a, h.b, n);
+}
+
+int Engine::pointer_device(const void* p) {
+  cudaPointerAttributes a;
+  if (!p || cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return -1; }
+  return (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) ? a.device : -1;
+}
+
+int Engine::current_device() {
+  int d = 0;
+  CK(cudaGetDevice(&d));
+  return d;
+}
+
+void Engine::free_device(void* p, void* user_stream) {
+  if (!p) return;
+  int prev = 0;
+  CK(cudaGetDevice(&prev));
+  const int d = pointer_device(p);
+  if (d >= 0) CK(cudaSetDevice(d));  // a NULL stream is the legacy stream of the device that owns p
+  CK(cudaFreeAsync(p, (cudaStream_t)user_stream));
+  CK(cudaSetDevice(prev));
 }
 
 void Engine::parse(const std::vector<ParseRange>& ranges, ParseResult& out, int lane_id) {
@@ -1196,6 +1290,45 @@ void Engine::emit(const std::vector<EmitPiece>& pieces, uint64_t total_bits, uin
   if (nbytes == 0) return;
   const void* d = emit_device(pieces, total_bits, 0);
   download(d, host_dst, nbytes);
+}
+
+uint8_t* Engine::emit_to_device(const std::vector<EmitPiece>& pieces, uint64_t total_bits, const uint8_t* hdr,
+                                int hdr_len, int checksum, void* user_stream, size_t* outsize) {
+  const void* body = emit_device(pieces, total_bits, 0);
+  Impl& m = *p_;
+  Lane& l = m.lane[0];
+  std::lock_guard<std::mutex> g(l.mu);
+  CK(cudaSetDevice(m.dev));
+  const cudaStream_t us = (cudaStream_t)user_stream;
+  const size_t nbytes = (size_t)((total_bits + 7) / 8);
+  const size_t trailer = checksum == kCkCrc32 ? 8 : (checksum == kCkAdler32 ? 4 : 0);
+  const size_t total = (size_t)hdr_len + nbytes + trailer;
+  uint8_t* out = nullptr;
+  CK(cudaMallocAsync((void**)&out, total, us));
+  CK(cudaEventRecord(m.ev_user, us));  // the allocation exists before lane 0 writes into it
+  CK(cudaStreamWaitEvent(l.stream, m.ev_user, 0));
+  if (nbytes) CK(cudaMemcpyAsync(out + hdr_len, body, nbytes, cudaMemcpyDeviceToDevice, l.stream));
+  if (hdr_len || trailer) {
+    if (checksum != kCkNone) CK(cudaStreamWaitEvent(l.stream, m.ev_ck, 0));
+    ContainerArgs a;
+    memset(&a, 0, sizeof(a));
+    a.out = out;
+    a.body_bytes = nbytes;
+    a.isize = m.insize;
+    a.acc = m.ck_acc.as<ChecksumAcc>();
+    a.tab = Impl::crc_tab();
+    memcpy(a.hdr, hdr, (size_t)hdr_len);
+    a.hdr_len = (uint32_t)hdr_len;
+    a.kind = checksum;
+    k_container<<<1, 32, 0, l.stream>>>(a);
+    CK(cudaGetLastError());
+    l.acc.launches++;
+  }
+  CK(cudaEventRecord(m.ev_lane0, l.stream));
+  CK(cudaStreamWaitEvent(us, m.ev_lane0, 0));
+  l.sync();
+  *outsize = total;
+  return out;
 }
 
 uint64_t Engine::device_block_bits(const uint32_t* hist320) {

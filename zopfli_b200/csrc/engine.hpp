@@ -60,6 +60,19 @@ class Engine {
   // 16 bytes past insize (e.g. a padded torch tensor).
   void set_input_host(const uint8_t* in, size_t insize);
   void set_input_device(const uint8_t* dev_in, size_t insize);
+  // Device bytes of any alignment (nothing past insize is read), copied device to device after the work
+  // queued on user_stream (cudaStream_t of this context's device, NULL = legacy default stream).
+  // checksum (checksum.hpp ChecksumKind: 0 CRC-32, 1 Adler-32, 2 none) starts on a stream of its own
+  // beside the parse; its result stays on the device for emit_to_device.
+  void set_input_device_copy(const uint8_t* dev_src, size_t insize, void* user_stream, int checksum);
+  // CRC-32 / Adler-32 (ChecksumKind) of dev_in[0, n) computed on the device, after the work queued on
+  // user_stream; blocks until the result is known.
+  uint32_t checksum_device(const uint8_t* dev_in, size_t n, void* user_stream, int checksum);
+  // device that owns p (device or managed memory), else -1
+  static int pointer_device(const void* p);
+  static int current_device();
+  // cudaFreeAsync of an allocation made by emit_to_device
+  static void free_device(void* p, void* user_stream);
 
   // `lane` selects one of kLanes independent stream + arena sets; calls on different lanes may run
   // concurrently from different host threads (chunk pipelines; giant blocks beside the rest).
@@ -126,6 +139,11 @@ class Engine {
   // the emitted size) and returns its device address; download() copies device bytes to the host.
   void* emit_device(const std::vector<EmitPiece>& pieces, uint64_t total_bits, size_t reserve_bytes);
   void download(const void* dev_src, uint8_t* host_dst, size_t nbytes);
+  // emit() into device memory: a fresh cudaMallocAsync allocation on user_stream of *outsize bytes holding
+  // hdr[0, hdr_len), the stream (bit phase 0) and the trailer of `checksum` (the one started by
+  // set_input_device_copy) with ISIZE = the input size.  user_stream waits for the result; the caller owns it.
+  uint8_t* emit_to_device(const std::vector<EmitPiece>& pieces, uint64_t total_bits, const uint8_t* hdr, int hdr_len,
+                          int checksum, void* user_stream, size_t* outsize);
   // host -> device through the context's threaded pinned staging (synchronous)
   void upload(void* dev_dst, const uint8_t* host_src, size_t nbytes);
   void* stream();   // cudaStream_t of lane 0, the stream emit / download / set_input run on
