@@ -184,15 +184,9 @@ ZB_HD unsigned clcl_rank_symbol(unsigned k) {  // RFC1951 3.2.7 transmission ord
   return (k & 1) ? 7 - h : 8 + h;
 }
 
-// EncodeTree with out == NULL (deflate.c:105-249): bits of the tree header for one flag choice
-template <typename LenT>
-ZB_HD uint32_t encode_tree_size(const LenT* ll_lengths, const LenT* d_lengths, bool use_16,
-                                bool use_17, bool use_18) {
-  uint32_t clcounts[19];
-  for (int i = 0; i < 19; i++) clcounts[i] = 0;
-  const TreeShape sh = tree_shape(ll_lengths, d_lengths);
-  tree_tokens(ll_lengths, d_lengths, sh, (use_16 ? 1u : 0u) | (use_17 ? 2u : 0u) | (use_18 ? 4u : 0u),
-              [&](unsigned sym, unsigned) { clcounts[sym]++; });
+// The rest of EncodeTree(size_only) once the code-length-code counts are known (deflate.c:205-241):
+// their length-limited code, HCLEN, and the bits of the header
+ZB_HD uint32_t tree_header_bits(const uint32_t* clcounts) {
   uint8_t clcl[19];
   PmScratch<19, 7> s;
   length_limited<19, 7>(clcounts, 19, 7, clcl, s);
@@ -202,6 +196,51 @@ ZB_HD uint32_t encode_tree_size(const LenT* ll_lengths, const LenT* d_lengths, b
   for (int i = 0; i < 19; i++) r += clcl[i] * clcounts[i];
   r += clcounts[16] * 2 + clcounts[17] * 3 + clcounts[18] * 7;
   return r;
+}
+
+// EncodeTree with out == NULL (deflate.c:105-249): bits of the tree header for one flag choice
+template <typename LenT>
+ZB_HD uint32_t encode_tree_size(const LenT* ll_lengths, const LenT* d_lengths, bool use_16,
+                                bool use_17, bool use_18) {
+  uint32_t clcounts[19];
+  for (int i = 0; i < 19; i++) clcounts[i] = 0;
+  const TreeShape sh = tree_shape(ll_lengths, d_lengths);
+  tree_tokens(ll_lengths, d_lengths, sh, (use_16 ? 1u : 0u) | (use_17 ? 2u : 0u) | (use_18 ? 4u : 0u),
+              [&](unsigned sym, unsigned) { clcounts[sym]++; });
+  return tree_header_bits(clcounts);
+}
+
+// Code-length-code counts that tree_tokens produces for one maximal run of c equal lengths v (a run
+// in the transmitted sequence ll_len[0 .. hlit+257) ++ d_len[0 .. hdist+1)) under `flags`, added
+// through add(sym, count).  tree_tokens only extends a run where a repeat code could use it; where it
+// does not, each length of the run is a token of its own, which is the c literal tokens below.
+template <typename Add>
+ZB_HD void run_token_counts(unsigned v, unsigned c, unsigned flags, Add add) {
+  const bool use_16 = (flags & 1) != 0, use_17 = (flags & 2) != 0, use_18 = (flags & 4) != 0;
+  if (!(use_16 || (v == 0 && (use_17 || use_18)))) { add(v, c); return; }
+  if (v == 0) {
+    if (use_18 && c >= 11) {
+      unsigned n = c / 138;
+      c %= 138;
+      if (c >= 11) { n++; c = 0; }
+      add(18u, n);
+    }
+    if (use_17 && c >= 3) {
+      unsigned n = c / 10;
+      c %= 10;
+      if (c >= 3) { n++; c = 0; }
+      add(17u, n);
+    }
+  }
+  if (use_16 && c >= 4) {
+    add(v, 1u);
+    c--;
+    unsigned n = c / 6;
+    c %= 6;
+    if (c >= 3) { n++; c = 0; }
+    add(16u, n);
+  }
+  if (c) add(v, c);
 }
 
 // deflate.c:277-290 / 251-272: first minimum over the 8 flag combinations.

@@ -460,14 +460,26 @@ void deflate_units(Engine& eng, const ZopfliOptions* opt, int btype, bool final_
       parse_lane(1, lane_r);
       debug_mark(cid, "C rest parsed");
       add_time(g_host_times.other, now_ms() - t0);
+      // A master block with a giant also has blocks on lane_r, so its D-E waits for both lanes.  The
+      // clean and the dirty D-E then run side by side, each on its own lane: their second split searches
+      // are chains of short, latency-bound rounds that leave most of the GPU idle, and when the giants end
+      // before the rest the dirty D-E no longer queues behind the clean one.  With verbose output the two
+      // run in turn, so the split-point reports keep their order (clean master blocks first).
+      auto dirty_tail = [&] {
+        double tw = now_ms();
+        tg.join();
+        debug_mark(cid, "C giants parsed");
+        add_time(g_host_times.other, now_ms() - tw);
+        finish(dirty, lane_g);  // the giants' lane is idle now and has stream priority
+        debug_mark(cid, "D-E dirty done");
+      };
+      const bool in_turn = opt->verbose || opt->verbose_more;
+      std::thread td;
+      if (!in_turn) td = std::thread(dirty_tail);
       finish(clean, lane_r);   // overlaps the giants' DP chains still running on lane_g
       debug_mark(cid, "D-E clean done");
-      double tw = now_ms();
-      tg.join();
-      debug_mark(cid, "C giants parsed");
-      add_time(g_host_times.other, now_ms() - tw);
-      finish(dirty, lane_g);  // the giants' lane is idle now and has stream priority
-      debug_mark(cid, "D-E dirty done");
+      if (in_turn) dirty_tail();
+      else td.join();
     }
   }
   };  // run_chunk

@@ -394,6 +394,49 @@ __device__ __noinline__ void warp_length_limited(const uint32_t* freq, int n, ui
 // code-length set (cs.len[choice->set]) and the tree flags that realise the size are reported too
 // (what AddDynamicTree / GetDynamicLengths would pick: first minimum of the 8 flag combinations).
 struct DynChoice { uint32_t set, flags, tree_bits; };
+
+// Tree-header bits of both code-length sets (cs.len[0], cs.len[1]) under all 8 flag combinations
+// (EncodeTree size_only, deflate.c:105-249): lane l < 16 returns the size for set l >> 3, flags l & 7.
+// The token counts are summed per maximal run of equal lengths (run_token_counts), with the runs of
+// each set spread over the warp, instead of 16 lanes walking the sequence one length at a time down
+// eight diverging paths.  The counts, and so the sizes, are those encode_tree_size computes.
+__device__ __noinline__ uint32_t warp_tree_sizes(CostStage& cs, uint32_t lane) {
+  uint32_t* cl = &cs.pm.row[0][0];   // [set][flags][19] counts; the package-merge rows are free by now
+  uint32_t* starts = cs.pm.mask[0];  // run starts of one set, a bit per position
+  for (int i = lane; i < 2 * 8 * 19; i += 32) cl[i] = 0;
+  for (int set = 0; set < 2; set++) {
+    const uint8_t* ll = cs.len[set];
+    const uint8_t* dl = ll + 288;
+    const TreeShape sh = tree_shape(ll, dl);
+    const unsigned nll = sh.hlit + 257, nwords = (sh.total + 31) >> 5;
+    auto at = [&](unsigned i) -> unsigned { return i < nll ? ll[i] : dl[i - nll]; };
+    __syncwarp();
+    for (unsigned w = 0; w < nwords; w++) {
+      const unsigned i = w * 32 + lane;
+      const bool st = i < sh.total && (i == 0 || at(i) != at(i - 1));
+      const uint32_t m = __ballot_sync(0xffffffffu, st);
+      if (lane == 0) starts[w] = m;
+    }
+    __syncwarp();
+    for (unsigned i = lane; i < sh.total; i += 32) {
+      const unsigned b = i & 31;
+      unsigned w = i >> 5;
+      if (!((starts[w] >> b) & 1u)) continue;
+      unsigned end = sh.total;   // the run ends at the next run start
+      uint32_t m = b == 31 ? 0u : starts[w] & ~((2u << b) - 1u);
+      while (!m && ++w < nwords) m = starts[w];
+      if (m) end = w * 32 + (unsigned)(__ffs(m) - 1);
+      const unsigned v = at(i), c = end - i;
+      for (unsigned f = 0; f < 8; f++) {
+        uint32_t* dst = cl + (set * 8 + f) * 19;
+        run_token_counts(v, c, f, [&](unsigned sym, unsigned n) { atomicAdd(&dst[sym], n); });
+      }
+    }
+  }
+  __syncwarp();
+  return lane < 16 ? tree_header_bits(cl + lane * 19) : 0xffffffffu;
+}
+
 __device__ uint64_t warp_dynamic_bits(const uint32_t* hist, CostStage& cs, uint32_t lane, DynChoice* choice = nullptr) {
   // RLE-smoothed copies of both histograms (TryOptimizeHuffmanForRle deflate.c:525-567): two
   // serial scans side by side, then four warp-wide code constructions
@@ -407,12 +450,8 @@ __device__ uint64_t warp_dynamic_bits(const uint32_t* hist, CostStage& cs, uint3
   warp_length_limited(cs.cnt2 + 288, kNumD, cs.len[1] + 288, cs.pm, lane);
   if (lane < 2) patch_distance_codes(cs.len[lane] + 288);
   __syncwarp();
-  uint32_t tsz = 0xffffffffu;
-  if (lane < 16) {
-    const uint8_t* l = cs.len[lane >> 3];
-    tsz = encode_tree_size(l, l + 288, (lane & 1) != 0, (lane & 2) != 0, (lane & 4) != 0);
-    tsz = (tsz << 3) | (lane & 7u);  // ties go to the lowest flag index (deflate.c:259-267 keeps the first minimum)
-  }
+  uint32_t tsz = warp_tree_sizes(cs, lane);
+  if (lane < 16) tsz = (tsz << 3) | (lane & 7u);  // ties go to the lowest flag index (deflate.c:259-267 keeps the first minimum)
   // min over lanes 0..7 and 8..15 (deflate.c:277-290)
 #pragma unroll
   for (int d = 4; d > 0; d >>= 1) {
