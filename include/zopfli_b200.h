@@ -73,6 +73,27 @@ double ZopfliB200HostBlockSize(const unsigned char* in, const unsigned short* li
 uint64_t ZopfliB200HostEmitBlock(const unsigned char* in, const unsigned short* litlens,
                                  const unsigned short* dists, size_t n, size_t lstart, size_t lend,
                                  int btype, int final, unsigned char* out, size_t cap);
+/* AddLZ77Block (deflate.c:682-745) for a list of pieces of one LZ77 store, placed one after the other as
+ * the driver places blocks.  Piece i is symbols [lstart[i], lend[i]) of (litlens, dists), block type
+ * btype[i] (0 stored, 1 fixed, 2 dynamic) with BFINAL final[i].  The store's first symbol covers in[0]
+ * and the store covers at most insize bytes (stored pieces copy them).  The stream starts at bit bp0
+ * (0..7) of out[0], the bits before it zero; *nbits receives its end bit position, out (cap bytes) the
+ * bytes [0, ceil(*nbits / 8)).  Every piece gets a plan, the block plan the emission uses:
+ * plan_len[i*320 ..] its 288 + 32 dynamic code lengths, plan_val[i*6 ..] its tree flags (use_16 | use_17
+ * << 1 | use_18 << 2), tree-header bits, dynamic / fixed / stored block bits and input bytes.
+ * Device: the plan from k_block_plan, the stream from k_emit (product library only, like the device-memory
+ * calls below).  Host: their host twins (host_emit.hpp).
+ * Return 1 on invalid symbols or ranges or when the stream does not fit in cap (*nbits is set then). */
+int ZopfliB200DeviceEmitBlocks(const unsigned char* in, size_t insize, const unsigned short* litlens,
+                               const unsigned short* dists, size_t n, size_t npieces, const size_t* lstart,
+                               const size_t* lend, const int* btype, const int* final, unsigned bp0,
+                               unsigned char* out, size_t cap, uint64_t* nbits, unsigned char* plan_len,
+                               uint64_t* plan_val);
+int ZopfliB200HostEmitBlocks(const unsigned char* in, size_t insize, const unsigned short* litlens,
+                             const unsigned short* dists, size_t n, size_t npieces, const size_t* lstart,
+                             const size_t* lend, const int* btype, const int* final, unsigned bp0,
+                             unsigned char* out, size_t cap, uint64_t* nbits, unsigned char* plan_len,
+                             uint64_t* plan_val);
 /* OptimizeHuffmanForRle (deflate.c:434-518) as restated for host and device, in place, n <= 288. */
 void ZopfliB200HostOptimizeRle(uint32_t* counts, int n);
 /* ZopfliLengthLimitedCodeLengths (katajainen.h:35-36) as restated for host and device. */

@@ -1,6 +1,7 @@
 """ctypes bindings used by the tests only.
 
-  ref     -- the UNMODIFIED reference, oracle/_ref/libzopfli_ref.so (+ libref_seams.so wrappers)
+  ref     -- the UNMODIFIED reference, oracle/_ref/libzopfli_ref.so (+ libref_seams.so wrappers, and
+             libref_emit.so: deflate.c's static block emission, compiled in place)
   oracle  -- the plain-C restatement, oracle/_build/libzopfli_oracle.so
   digest / reference -- the reference's recorded outputs (tests/golden/reference_outputs.json), which the
              GPU tests compare against so that they run where the reference cannot be built
@@ -64,7 +65,8 @@ def ensure_built():
     need = [os.path.join(ORACLE_DIR, "_build", "libzopfli_oracle.so")]
     if os.path.isdir("/root/reference/src/zopfli"):
         need += [os.path.join(ORACLE_DIR, "_ref", "libzopfli_ref.so"),
-                 os.path.join(ORACLE_DIR, "_ref", "libref_seams.so")]
+                 os.path.join(ORACLE_DIR, "_ref", "libref_seams.so"),
+                 os.path.join(ORACLE_DIR, "_ref", "libref_emit.so")]
     if not all(os.path.exists(p) for p in need):
         subprocess.check_call(["make", "-s", "-C", ORACLE_DIR, "all"])
 
@@ -72,7 +74,7 @@ def ensure_built():
 def have_reference():
     """the compiled reference is present (oracle/Makefile builds it only where the reference's sources are)"""
     return all(os.path.exists(os.path.join(ORACLE_DIR, "_ref", n))
-               for n in ("libzopfli_ref.so", "libzopfli_ref_ndebug.so", "libref_seams.so"))
+               for n in ("libzopfli_ref.so", "libzopfli_ref_ndebug.so", "libref_seams.so", "libref_emit.so"))
 
 
 def _np_u8(b):
@@ -93,6 +95,12 @@ class Ref:
         name = "libzopfli_ref_ndebug.so" if ndebug else "libzopfli_ref.so"
         self.lib = C.CDLL(os.path.join(ORACLE_DIR, "_ref", name))
         self.seams = C.CDLL(os.path.join(ORACLE_DIR, "_ref", "libref_seams.so"))
+        self.emit = C.CDLL(os.path.join(ORACLE_DIR, "_ref", "libref_emit.so"))
+        self.emit.ref_emit_blocks.restype = C.c_size_t
+        self.emit.ref_emit_blocks.argtypes = [C.c_void_p] * 3 + [C.c_size_t] * 2 + [C.c_void_p] * 4 + \
+            [C.c_int, C.c_void_p, C.c_size_t, C.c_void_p]
+        self.emit.ref_encode_tree.restype = C.c_size_t
+        self.emit.ref_encode_tree.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_size_t]
         self.lib.ZopfliCompress.argtypes = [C.POINTER(ZopfliOptions), C.c_int, C.c_void_p, C.c_size_t,
                                             C.POINTER(C.c_void_p), C.POINTER(C.c_size_t)]
         self.lib.ZopfliCompress.restype = None
@@ -230,6 +238,31 @@ class Ref:
         c = np.array(counts, dtype=np.uint64)
         self.seams.ref_optimize_rle(len(c), c.ctypes.data)
         return c
+
+    def emit_blocks(self, data, litlens, dists, pieces, bp0=0):
+        """AddLZ77Block for each (lstart, lend, btype, final) piece of the store (litlens, dists), whose first
+        symbol covers data[0], from bit bp0 of a one-byte buffer (an empty one for bp0 = 0) -> (bytes, bp)"""
+        a = _np_u8(data)
+        ll = np.ascontiguousarray(litlens, dtype=np.uint16)
+        dd = np.ascontiguousarray(dists, dtype=np.uint16)
+        p = np.array(pieces, dtype=np.int64).reshape(-1, 4)
+        ls, le = np.ascontiguousarray(p[:, 0], np.uint64), np.ascontiguousarray(p[:, 1], np.uint64)
+        bt, fi = np.ascontiguousarray(p[:, 2], np.int32), np.ascontiguousarray(p[:, 3], np.int32)
+        cap = 6 * len(ll) + len(data) + 512 * len(p) + 5 * (len(data) // 65535 + len(p)) + 16
+        out = np.zeros(cap, dtype=np.uint8)
+        bp = C.c_ubyte(0)
+        n = self.emit.ref_emit_blocks(a.ctypes.data, ll.ctypes.data, dd.ctypes.data, len(ll), len(p), ls.ctypes.data,
+                                      le.ctypes.data, bt.ctypes.data, fi.ctypes.data, bp0, out.ctypes.data, cap,
+                                      C.byref(bp))
+        assert n <= cap
+        return out[:n].tobytes(), bp.value
+
+    def encode_tree(self, lengths320, flags):
+        """EncodeTree of 288 + 32 code lengths with flags use_16 | use_17 << 1 | use_18 << 2 -> (bits, bytes)"""
+        ln = np.ascontiguousarray(lengths320, dtype=np.uint32)
+        out = np.zeros(512, dtype=np.uint8)
+        bits = self.emit.ref_encode_tree(ln.ctypes.data, ln[288:].ctypes.data, flags, out.ctypes.data, len(out))
+        return int(bits), out[: (bits + 7) // 8].tobytes()
 
 
 class ZoStore(C.Structure):

@@ -50,7 +50,7 @@ EXPORTS = ["ZopfliInitOptions", "ZopfliCompress", "ZopfliDeflate", "ZopfliDeflat
            "ZopfliCalculateBlockSize", "ZopfliCalculateBlockSizeAutoType",
            "ZopfliGzipCompress", "ZopfliZlibCompress", "ZopfliB200LZ77", "ZopfliB200LZ77Batch",
            "ZopfliB200MatchTable", "ZopfliB200DynamicBlockBits", "ZopfliB200DeviceAutoTypeBits", "ZopfliB200HostBlockSplitLZ77",
-           "ZopfliB200HostBatchedSplit", "ZopfliB200HostBlockSize", "ZopfliB200HostEmitBlock", "ZopfliB200HostLengthLimited", "ZopfliB200HostOptimizeRle",
+           "ZopfliB200HostBatchedSplit", "ZopfliB200HostBlockSize", "ZopfliB200HostEmitBlock", "ZopfliB200DeviceEmitBlocks", "ZopfliB200HostEmitBlocks", "ZopfliB200HostLengthLimited", "ZopfliB200HostOptimizeRle",
            "ZopfliB200DeflateSpan", "ZopfliB200AppendSpan", "ZopfliB200LastMasterBitOffsets", "ZopfliB200Crc32", "ZopfliB200Crc32Combine", "ZopfliB200Adler32", "ZopfliB200CompressDevice",
            "ZopfliB200DistUniqueId", "ZopfliB200DistInit", "ZopfliB200DistCompress", "ZopfliB200DistFinalize", "ZopfliB200DistShard", "ZopfliB200DistPlacement",
            "ZopfliB200GetStats", "ZopfliB200ResetStats", "ZopfliB200SetStream", "ZopfliB200Device",
@@ -173,6 +173,8 @@ class Library:
         L.ZopfliB200HostBlockSize.restype = C.c_double
         L.ZopfliB200HostEmitBlock.argtypes = [vp, vp, vp, sz, sz, sz, C.c_int, C.c_int, vp, sz]
         L.ZopfliB200HostEmitBlock.restype = C.c_uint64
+        L.ZopfliB200HostEmitBlocks.argtypes = [vp, sz, vp, vp, sz, sz, vp, vp, vp, vp, C.c_uint, vp, sz, vp, vp, vp]
+        L.ZopfliB200HostEmitBlocks.restype = C.c_int
         L.ZopfliB200HostLengthLimited.argtypes = [vp, C.c_int, C.c_int, vp]
         L.ZopfliB200HostOptimizeRle.argtypes = [vp, C.c_int]
         L.ZopfliB200HostOptimizeRle.restype = None
@@ -190,12 +192,15 @@ class Library:
         L.ZopfliB200Adler32.restype = C.c_uint32
         L.ZopfliB200HostChecksumSliced.argtypes = [vp, sz, sz, C.c_int]
         L.ZopfliB200HostChecksumSliced.restype = C.c_uint32
-        # device-resident calls (csrc/device_api.cpp); a host-only test build of the ABI does not export them
+        # device-resident calls and the device emission seam (csrc/device_api.cpp); a host-only test build of the
+        # ABI does not export them
         for name, args, res in (("ZopfliB200CompressDeviceToDevice",
                                  [C.POINTER(ZopfliOptions), C.c_int, vp, sz, vp, C.POINTER(vp), C.POINTER(sz)], C.c_int),
                                 ("ZopfliB200FreeDevice", [vp, vp], None),
                                 ("ZopfliB200Crc32Device", [vp, sz, vp, C.POINTER(C.c_uint32)], C.c_int),
-                                ("ZopfliB200Adler32Device", [vp, sz, vp, C.POINTER(C.c_uint32)], C.c_int)):
+                                ("ZopfliB200Adler32Device", [vp, sz, vp, C.POINTER(C.c_uint32)], C.c_int),
+                                ("ZopfliB200DeviceEmitBlocks", [vp, sz, vp, vp, sz, sz, vp, vp, vp, vp, C.c_uint, vp, sz, vp, vp,
+                                                                vp], C.c_int)):
             f = getattr(L, name, None)
             if f is not None:
                 f.argtypes, f.restype = args, res
@@ -360,6 +365,33 @@ class Library:
         bits = self.lib.ZopfliB200HostEmitBlock(None, ll.ctypes.data, dd.ctypes.data, len(ll), lstart, lend,
                                                 btype, final, out.ctypes.data, cap)
         return out[: (bits + 7) // 8].tobytes(), int(bits)
+
+    def emit_blocks(self, data, litlens, dists, pieces, bp0=0, device=True):
+        """ZopfliB200DeviceEmitBlocks (device=True: k_block_plan + k_emit) or ZopfliB200HostEmitBlocks (their
+        host twins).  pieces: (lstart, lend, btype, final) symbol ranges of the store (litlens, dists), whose
+        first symbol covers data[0].  Returns (stream bytes, end bit position, plans); the stream starts at
+        bit bp0 of its first byte.  plans: one dict per piece with "len" (288 + 32 code lengths), "flags",
+        "tree_bits", "dyn_bits", "fixed_bits", "unc_bits" and "nbytes"."""
+        a = _pad(data)
+        ll = np.ascontiguousarray(litlens, np.uint16)
+        dd = np.ascontiguousarray(dists, np.uint16)
+        p = np.array(pieces, np.int64).reshape(-1, 4)
+        ls, le = np.ascontiguousarray(p[:, 0], np.uint64), np.ascontiguousarray(p[:, 1], np.uint64)
+        bt, fi = np.ascontiguousarray(p[:, 2], np.int32), np.ascontiguousarray(p[:, 3], np.int32)
+        cap = 6 * len(ll) + len(data) + 512 * len(p) + 5 * (len(data) // 65535 + len(p)) + 16
+        out = np.zeros(cap, np.uint8)
+        nbits = C.c_uint64(0)
+        lens = np.zeros((len(p), 320), np.uint8)
+        vals = np.zeros((len(p), 6), np.uint64)
+        fn = self.lib.ZopfliB200DeviceEmitBlocks if device else self.lib.ZopfliB200HostEmitBlocks
+        rc = fn(a.ctypes.data, len(data), ll.ctypes.data, dd.ctypes.data, len(ll), len(p), ls.ctypes.data,
+                le.ctypes.data, bt.ctypes.data, fi.ctypes.data, bp0, out.ctypes.data, cap, C.byref(nbits),
+                lens.ctypes.data, vals.ctypes.data)
+        if rc != 0:
+            raise ValueError("emit_blocks: invalid symbols or pieces")
+        names = ("flags", "tree_bits", "dyn_bits", "fixed_bits", "unc_bits", "nbytes")
+        plans = [dict({"len": lens[i].copy()}, **{k: int(v) for k, v in zip(names, vals[i])}) for i in range(len(p))]
+        return out[: (nbits.value + 7) // 8].tobytes(), int(nbits.value), plans
 
     def host_optimize_rle(self, counts):
         c = np.ascontiguousarray(counts, np.uint32).copy()

@@ -64,6 +64,40 @@ int container_header(ZopfliFormat fmt, unsigned char* hdr) {
   return 0;
 }
 
+bool seam_pieces(size_t insize, const unsigned short* ll, const unsigned short* d, size_t n, size_t npieces,
+                 const size_t* lstart, const size_t* lend, const int* btype, const int* final, unsigned bp0,
+                 std::vector<Piece>& pieces) {
+  if (bp0 > 7) return false;
+  std::vector<uint64_t> pos(n + 1, 0);
+  for (size_t i = 0; i < n; i++) {
+    if (d[i] == 0 ? ll[i] > 255 : (ll[i] < 3 || ll[i] > 258 || d[i] > 32768)) return false;
+    pos[i + 1] = pos[i] + (d[i] == 0 ? 1 : ll[i]);
+  }
+  if (pos[n] > insize) return false;
+  pieces.assign(npieces, Piece());
+  for (size_t i = 0; i < npieces; i++) {
+    if (lstart[i] > lend[i] || lend[i] > n || btype[i] < 0 || btype[i] > 2) return false;
+    Piece& p = pieces[i];
+    p.type = (uint8_t)btype[i];
+    p.final = final[i] != 0;
+    p.buf = Engine::kFin;
+    p.off = lstart[i];
+    p.n = (uint32_t)(lend[i] - lstart[i]);
+    p.instart = (size_t)pos[lstart[i]];
+    p.inend = (size_t)pos[lend[i]];
+  }
+  return true;
+}
+
+void seam_plan_out(const BlockPlan& b, Piece& p, unsigned char* len320, uint64_t* val6) {
+  memcpy(len320, b.ll_len, kNumLL);
+  memcpy(len320 + kNumLL, b.d_len, kNumD);
+  const uint64_t v[6] = {b.tree_flags, b.tree_bits, b.dyn_bits, b.fixed_bits, b.unc_bits, b.nbytes};
+  memcpy(val6, v, sizeof(v));
+  p.nbits = p.type == 1 ? b.fixed_bits : b.dyn_bits;
+  p.tree_bits = b.tree_bits;
+}
+
 }  // namespace zb
 
 namespace {
@@ -569,6 +603,37 @@ uint64_t ZopfliB200HostEmitBlock(const unsigned char* in, const unsigned short* 
   if (nbits != want) { fprintf(stderr, "zopfli-b200: emitted %llu bits, predicted %llu\n", (unsigned long long)nbits, (unsigned long long)want); abort(); }
   if ((nbits + 7) / 8 <= cap) memcpy(out, buf.data(), (size_t)((nbits + 7) / 8));
   return nbits;
+}
+
+int ZopfliB200HostEmitBlocks(const unsigned char* in, size_t insize, const unsigned short* litlens,
+                             const unsigned short* dists, size_t n, size_t npieces, const size_t* lstart,
+                             const size_t* lend, const int* btype, const int* final, unsigned bp0,
+                             unsigned char* out, size_t cap, uint64_t* nbits, unsigned char* plan_len,
+                             uint64_t* plan_val) {
+  std::vector<Piece> pieces;
+  if (!seam_pieces(insize, litlens, dists, n, npieces, lstart, lend, btype, final, bp0, pieces)) return 1;
+  std::vector<BlockPlan> plans(npieces);
+  for (size_t i = 0; i < npieces; i++) {
+    host_block_plan(litlens + pieces[i].off, dists + pieces[i].off, pieces[i].n, plans[i]);
+    seam_plan_out(plans[i], pieces[i], plan_len + i * 320, plan_val + i * 6);
+  }
+  std::vector<Engine::EmitPiece> ep;
+  *nbits = layout_pieces(pieces, 0, bp0, ep, nullptr);
+  const size_t nbytes = (size_t)((*nbits + 7) / 8);
+  if (nbytes > cap) return 1;
+  std::vector<uint8_t> buf(nbytes + 16, 0);
+  for (size_t i = 0; i < npieces; i++) {
+    const Engine::EmitPiece& e = ep[i];
+    HostBitSink sink{buf.data(), e.bit_start};
+    if (e.type == 0) {
+      host_emit_stored(e.final != 0, in + e.in_start, e.in_len, sink);
+      continue;
+    }
+    const uint64_t nb = host_emit_block(e.type, e.final != 0, litlens + e.off, dists + e.off, e.n, &plans[i], sink);
+    if (nb != e.nbits) { fprintf(stderr, "zopfli-b200: emitted %llu bits, predicted %llu\n", (unsigned long long)nb, (unsigned long long)e.nbits); abort(); }
+  }
+  memcpy(out, buf.data(), nbytes);
+  return 0;
 }
 
 int ZopfliB200HostLengthLimited(const uint32_t* freq, int n, int maxbits, unsigned* bitlengths) {

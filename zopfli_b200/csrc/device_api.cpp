@@ -1,6 +1,8 @@
 // C-ABI calls of libzopfli.so.1 whose input and result live in device memory (include/zopfli_b200.h,
 // "input and output in device memory"): the deflate pieces are the ones ZopfliCompress produces, the stream
 // is emitted behind the container header in a device allocation, and the checksum is computed on the device.
+// Also the device half of the block-emission seam (ZopfliB200DeviceEmitBlocks), which needs engine calls
+// the host-only test build of api.cpp does not have.
 #include <stdio.h>
 
 #include <vector>
@@ -9,6 +11,7 @@
 #include "api.hpp"
 #include "checksum.hpp"
 #include "driver.hpp"
+#include "emit_bits.hpp"
 #include "engine.hpp"
 
 using namespace zb;
@@ -75,6 +78,34 @@ int ZopfliB200Crc32Device(const unsigned char* dev_in, size_t size, void* cuda_s
 
 int ZopfliB200Adler32Device(const unsigned char* dev_in, size_t size, void* cuda_stream, uint32_t* adler) {
   return device_checksum(dev_in, size, cuda_stream, kCkAdler32, adler);
+}
+
+int ZopfliB200DeviceEmitBlocks(const unsigned char* in, size_t insize, const unsigned short* litlens,
+                               const unsigned short* dists, size_t n, size_t npieces, const size_t* lstart,
+                               const size_t* lend, const int* btype, const int* final, unsigned bp0,
+                               unsigned char* out, size_t cap, uint64_t* nbits, unsigned char* plan_len,
+                               uint64_t* plan_val) {
+  std::vector<Piece> pieces;
+  if (!seam_pieces(insize, litlens, dists, n, npieces, lstart, lend, btype, final, bp0, pieces)) return 1;
+  Engine::Lease eng;
+  eng->set_input_host(in, insize);
+  eng->load_symbols(Engine::kFin, litlens, dists, n);
+  std::vector<Engine::PlanReq> rq(npieces);
+  for (size_t i = 0; i < npieces; i++) rq[i] = {pieces[i].off, pieces[i].n, (uint32_t)Engine::kFin};
+  std::vector<Engine::PlanCost> costs;
+  std::vector<uint64_t> handles;
+  eng->plan_blocks(rq, costs, handles);
+  for (size_t i = 0; i < npieces; i++) {
+    BlockPlan b;
+    eng->download((const void*)(uintptr_t)handles[i], (uint8_t*)&b, sizeof(b));
+    pieces[i].plan = handles[i];
+    seam_plan_out(b, pieces[i], plan_len + i * 320, plan_val + i * 6);
+  }
+  std::vector<Engine::EmitPiece> ep;
+  *nbits = layout_pieces(pieces, 0, bp0, ep, nullptr);  // the driver's placement: prefix sum, stored_end
+  if ((*nbits + 7) / 8 > cap) return 1;
+  eng->emit(ep, *nbits, out);
+  return 0;
 }
 
 }  // extern "C"

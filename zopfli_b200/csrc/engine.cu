@@ -94,6 +94,11 @@ struct LogService {
       fill(host, 0, kLogTabN);
     });
   }
+  // A process whose engines never parse (emission, checksums, block sizes only) never joins the filler in
+  // get(); a joinable std::thread destroyed at exit would call std::terminate.
+  ~LogService() {
+    if (filler.joinable()) filler.join();
+  }
   // table with at least need_n entries on `device`.  The default 2^21 entries cover every count a master
   // block can produce (symbols <= 10^6, blended statistics < 2x that); larger single ranges
   // (ZopfliDeflatePart with block splitting off) grow the table on demand.  An outgrown device copy is
@@ -1283,6 +1288,15 @@ void Engine::upload(void* dev_dst, const uint8_t* host_src, size_t nbytes) {
   m.stager.copy((uint8_t*)dev_dst, host_src, nbytes, true, m.dev);
   std::lock_guard<std::mutex> g(m.mu);
   m.st_acc.h2d_bytes += nbytes;
+}
+
+void Engine::load_symbols(int buf, const uint16_t* ll, const uint16_t* d, size_t n) {
+  Impl& m = *p_;
+  CK(cudaSetDevice(m.dev));
+  if (n > m.insize) { fprintf(stderr, "zopfli-b200: more symbols than input bytes\n"); abort(); }
+  m.ensure_sym(buf);
+  upload(m.sym_ll[buf].p, (const uint8_t*)ll, n * 2);
+  upload(m.sym_d[buf].p, (const uint8_t*)d, n * 2);
 }
 
 void Engine::emit(const std::vector<EmitPiece>& pieces, uint64_t total_bits, uint8_t* host_dst) {

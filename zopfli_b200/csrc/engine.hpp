@@ -146,6 +146,8 @@ class Engine {
                           int checksum, void* user_stream, size_t* outsize);
   // host -> device through the context's threaded pinned staging (synchronous)
   void upload(void* dev_dst, const uint8_t* host_src, size_t nbytes);
+  // test seam: symbols [0, n) of buffer `buf` (StoreBuf) from host arrays; n <= input size
+  void load_symbols(int buf, const uint16_t* ll, const uint16_t* d, size_t n);
   void* stream();   // cudaStream_t of lane 0, the stream emit / download / set_input run on
   uint64_t input_size() const;
   uint64_t device_memory_total() const;   // bytes of device memory (sizes the master-block batches of a pipeline)
