@@ -7,7 +7,6 @@
 #include <string.h>
 
 #include <algorithm>
-#include <chrono>
 #include <mutex>
 #include <thread>
 #include <vector>
@@ -27,10 +26,6 @@ using namespace zb;
 
 namespace {
 
-double now_ms() {
-  using namespace std::chrono;
-  return duration<double, std::milli>(steady_clock::now().time_since_epoch()).count();
-}
 std::mutex g_api_mu;   // guards g_total_ms and g_last_layout
 double g_total_ms = 0;
 std::vector<uint64_t> g_last_layout;  // bit offset of every unit (master block) of the most recent deflate call
@@ -38,8 +33,6 @@ std::vector<uint64_t> g_last_layout;  // bit offset of every unit (master block)
 }  // namespace
 
 namespace zb {
-
-double api_now_ms() { return now_ms(); }
 
 void api_call_done(std::vector<uint64_t>& layout, double t0) {
   std::lock_guard<std::mutex> g(g_api_mu);
@@ -62,6 +55,16 @@ int container_header(ZopfliFormat fmt, unsigned char* hdr) {
     return 2;
   }
   return 0;
+}
+
+void report_size(ZopfliFormat fmt, size_t insize, size_t outsize) {
+  const double removed = 100.0 * (double)(insize - outsize) / (double)insize;
+  if (fmt == ZOPFLI_FORMAT_DEFLATE)  // deflate.c:925-928
+    fprintf(stderr, "Original Size: %lu, Deflate: %lu, Compression: %f%% Removed\n", (unsigned long)insize,
+            (unsigned long)outsize, removed);
+  else  // gzip_container.c:118-122, zlib_container.c:73-77
+    fprintf(stderr, "Original Size: %d, %s: %d, Compression: %f%% Removed\n", (int)insize,
+            fmt == ZOPFLI_FORMAT_GZIP ? "Gzip" : "Zlib", (int)outsize, removed);
 }
 
 bool seam_pieces(size_t insize, const unsigned short* ll, const unsigned short* d, size_t n, size_t npieces,
@@ -179,32 +182,6 @@ uint32_t adler32(const unsigned char* data, size_t size) {
   return (uint32_t)((s2 << 16) | s1);
 }
 
-std::vector<std::pair<size_t, size_t>> master_units(size_t insize, size_t mb_begin, size_t mb_end) {
-  std::vector<std::pair<size_t, size_t>> u;
-  for (size_t m = mb_begin; m < mb_end; m++) {
-    size_t a = m * (size_t)kMasterBlock, b = a + kMasterBlock;
-    if (b > insize) b = insize;
-    u.push_back({a, b});
-  }
-  return u;
-}
-size_t num_master_blocks(size_t insize) {  // deflate.c:912-924 do/while
-  return insize == 0 ? 1 : (insize + kMasterBlock - 1) / kMasterBlock;
-}
-
-}  // namespace
-
-std::vector<std::pair<size_t, size_t>> zb::api_master_units(size_t insize) {
-  return master_units(insize, 0, num_master_blocks(insize));
-}
-
-namespace {
-
-bool api_debug() {
-  static int v = [] { const char* e = getenv("ZOPFLI_B200_DEBUG"); return e && atoi(e) ? 1 : 0; }();
-  return v != 0;
-}
-
 void deflate_impl(const ZopfliOptions* options, int btype, int final, const unsigned char* in,
                   size_t insize, const unsigned char* dev_in, unsigned char* bp, unsigned char** out,
                   size_t* outsize) {
@@ -222,17 +199,14 @@ void deflate_impl(const ZopfliOptions* options, int btype, int final, const unsi
   if (dev_in) eng->set_input_device(dev_in, insize);
   else eng->set_input_host(in, insize);
   const double t1 = now_ms();
-  deflate_units(*eng, options, btype, final != 0, in, master_units(insize, 0, num_master_blocks(insize)), 0, pieces);
+  deflate_units(*eng, options, btype, final != 0, master_blocks(0, insize), 0, pieces);
   const double t2 = now_ms();
   std::vector<uint64_t> layout;
   assemble(*eng, pieces, 0, bp, out, outsize, &layout, options->verbose != 0);
   { std::lock_guard<std::mutex> g(g_api_mu); g_last_layout.swap(layout); }
-  if (api_debug())
+  if (debug_on())
     fprintf(stderr, "[zb] api: set_input %.1f ms, deflate_units %.1f ms, emit %.1f ms\n", t1 - t0, t2 - t1, now_ms() - t2);
-  if (options->verbose) {
-    fprintf(stderr, "Original Size: %lu, Deflate: %lu, Compression: %f%% Removed\n", (unsigned long)insize,
-            (unsigned long)(*outsize - offset), 100.0 * (double)(insize - (*outsize - offset)) / (double)insize);
-  }
+  if (options->verbose) report_size(ZOPFLI_FORMAT_DEFLATE, insize, *outsize - offset);
   { std::lock_guard<std::mutex> g(g_api_mu); g_total_ms += now_ms() - t0; }
 }
 
@@ -252,41 +226,26 @@ template <typename Body>
 void container_impl(const ZopfliOptions* options, ZopfliFormat fmt, const unsigned char* in, size_t insize,
                     unsigned char** out, size_t* outsize, Body body) {
   unsigned char bp = 0;
-  unsigned char hdr[10];
-  if (fmt == ZOPFLI_FORMAT_GZIP) {  // gzip_container.c:84-124
-    uint32_t crc = 0;
-    std::thread crc_thread([&] { crc = crc32_parallel(in, insize); });  // overlaps the GPU work
-    append_bytes(hdr, container_header(fmt, hdr), out, outsize);
+  if (fmt == ZOPFLI_FORMAT_DEFLATE) {
     body(&bp);
-    const double tj = now_ms();
-    crc_thread.join();
-    if (api_debug()) fprintf(stderr, "[zb] api: crc join waited %.1f ms\n", now_ms() - tj);
-    unsigned char tr[8] = {(unsigned char)(crc & 255), (unsigned char)((crc >> 8) & 255),
-                           (unsigned char)((crc >> 16) & 255), (unsigned char)((crc >> 24) & 255),
-                           (unsigned char)(insize & 255), (unsigned char)((insize >> 8) & 255),
-                           (unsigned char)((insize >> 16) & 255), (unsigned char)((insize >> 24) & 255)};
-    append_bytes(tr, 8, out, outsize);
-    if (options->verbose)
-      fprintf(stderr, "Original Size: %d, Gzip: %d, Compression: %f%% Removed\n", (int)insize, (int)*outsize,
-              100.0 * (double)(insize - *outsize) / (double)insize);
-  } else if (fmt == ZOPFLI_FORMAT_ZLIB) {  // zlib_container.c:50-79
-    uint32_t checksum = 0;
-    std::thread adler_thread([&] { checksum = adler32(in, insize); });  // overlaps the GPU work
-    append_bytes(hdr, container_header(fmt, hdr), out, outsize);
-    body(&bp);
-    adler_thread.join();
-    unsigned char tr[4] = {(unsigned char)((checksum >> 24) & 255), (unsigned char)((checksum >> 16) & 255),
-                           (unsigned char)((checksum >> 8) & 255), (unsigned char)(checksum & 255)};
-    append_bytes(tr, 4, out, outsize);
-    if (options->verbose)
-      fprintf(stderr, "Original Size: %d, Zlib: %d, Compression: %f%% Removed\n", (int)insize, (int)*outsize,
-              100.0 * (double)(insize - *outsize) / (double)insize);
-  } else if (fmt == ZOPFLI_FORMAT_DEFLATE) {
-    body(&bp);
-  } else {
+    return;
+  }
+  if (fmt != ZOPFLI_FORMAT_GZIP && fmt != ZOPFLI_FORMAT_ZLIB) {
     fprintf(stderr, "zopfli-b200: unknown output format %d\n", (int)fmt);  // zopfli_lib.c:40 assert(0)
     abort();
   }
+  // gzip_container.c:84-124, zlib_container.c:50-79
+  const ChecksumKind kind = fmt == ZOPFLI_FORMAT_GZIP ? kCkCrc32 : kCkAdler32;
+  uint32_t sum = 0;
+  std::thread sum_thread([&] { sum = kind == kCkCrc32 ? crc32_parallel(in, insize) : adler32(in, insize); });  // overlaps the GPU work
+  unsigned char hdr[10], tr[8];
+  append_bytes(hdr, container_header(fmt, hdr), out, outsize);
+  body(&bp);
+  const double tj = now_ms();
+  sum_thread.join();
+  if (debug_on()) fprintf(stderr, "[zb] api: %s join waited %.1f ms\n", kind == kCkCrc32 ? "crc" : "adler", now_ms() - tj);
+  append_bytes(tr, container_trailer(kind, sum, insize, tr), out, outsize);
+  if (options->verbose) report_size(fmt, insize, *outsize);
 }
 
 void make_store(const unsigned short* ll, const unsigned short* dd, size_t n, Lz77Store& st) {
@@ -341,7 +300,7 @@ void ZopfliDeflatePart(const ZopfliOptions* options, int btype, int final, const
   std::vector<Piece> pieces;
   Engine::Lease eng;
   eng->set_input_host(in + base, inend - base);
-  deflate_units(*eng, options, btype, final != 0, in, {{instart, inend}}, base, pieces);
+  deflate_units(*eng, options, btype, final != 0, {{instart, inend}}, base, pieces);
   assemble(*eng, pieces, base, bp, out, outsize, nullptr, options->verbose != 0);
 }
 
@@ -362,12 +321,9 @@ int ZopfliB200DistCompress(const ZopfliOptions* options, ZopfliFormat output_typ
 int ZopfliB200DeflateSpan(const ZopfliOptions* options, const unsigned char* in, size_t insize,
                           const unsigned char* dev_in, size_t start, size_t end, int final,
                           unsigned char** span, size_t* spansize) {
-  std::vector<Piece> pieces;
-  std::vector<std::pair<size_t, size_t>> units;
   if (end > insize || start > end) return 1;
-  for (size_t a = start; a < end; a += kMasterBlock) units.push_back({a, a + kMasterBlock < end ? a + kMasterBlock : end});
-  if (units.empty() && insize == 0) units.push_back({0, 0});
-  if (units.empty()) return 0;
+  if (start == end && insize > 0) return 0;  // an empty span of an empty input is one empty master block
+  std::vector<Piece> pieces;
   size_t base = 0;
   Engine::Lease eng;
   if (dev_in) {
@@ -377,7 +333,7 @@ int ZopfliB200DeflateSpan(const ZopfliOptions* options, const unsigned char* in,
     base &= ~(size_t)15;
     eng->set_input_host(in + base, end - base);
   }
-  deflate_units(*eng, options, 2, final != 0, in, units, base, pieces);
+  deflate_units(*eng, options, 2, final != 0, master_blocks(start, end), base, pieces);
   // Records: maximal runs of compressed pieces, each emitted on the device from bit offset 0 of a
   // byte-aligned slot of one download buffer, and stored pieces as raw bytes.
   struct Rec { bool stored; bool final; size_t first, count; uint64_t bit0, nbits; };

@@ -4,7 +4,6 @@
 #include <stddef.h>
 #include <stdint.h>
 
-#include <utility>
 #include <vector>
 
 #include "../../include/zopfli.h"
@@ -14,14 +13,14 @@ namespace zb {
 struct BlockPlan;
 struct Piece;
 
-double api_now_ms();
-// the master blocks (deflate.c:908-931) of an insize-byte input, as ZopfliCompress cuts it
-std::vector<std::pair<size_t, size_t>> api_master_units(size_t insize);
-// a compression call that started at t0 (api_now_ms) is done: `layout` becomes what
+// a compression call that started at t0 (now_ms) is done: `layout` becomes what
 // ZopfliB200LastMasterBitOffsets returns, and the call's time is added to ZopfliB200Stats::ms_total
 void api_call_done(std::vector<uint64_t>& layout, double t0);
 // header bytes of the gzip or zlib container (at most 10); 0 for raw deflate
 int container_header(ZopfliFormat fmt, unsigned char* hdr);
+// the verbose report after the deflate body (fmt DEFLATE, outsize = its bytes) or after the gzip / zlib
+// container (outsize = the whole output buffer), in the reference's formats
+void report_size(ZopfliFormat fmt, size_t insize, size_t outsize);
 // The pieces of ZopfliB200{Device,Host}EmitBlocks as the driver describes blocks (kFin symbols, input bytes
 // for stored pieces); plan and nbits are filled in by the caller.  False if bp0 > 7, a symbol is not a valid
 // literal / (length, distance), a range lies outside the store, or the store covers more than insize bytes.

@@ -169,15 +169,10 @@ __global__ void k_container(ContainerArgs a) {
   const uint32_t lane = threadIdx.x;
   if (lane < a.hdr_len) a.out[lane] = a.hdr[lane];
   if (lane != 0) return;
-  uint8_t* tr = a.out + a.hdr_len + a.body_bytes;
-  if (a.kind == kCkCrc32) {
-    const uint32_t c = crc_finish(a.acc->crc0, a.isize, a.tab);
-    for (int k = 0; k < 4; k++) tr[k] = (uint8_t)(c >> (8 * k));
-    for (int k = 0; k < 4; k++) tr[4 + k] = (uint8_t)(a.isize >> (8 * k));
-  } else if (a.kind == kCkAdler32) {
-    const uint32_t c = adler_finish(a.acc->a, a.acc->b, a.isize);
-    for (int k = 0; k < 4; k++) tr[k] = (uint8_t)(c >> (24 - 8 * k));
-  }
+  const uint32_t c = a.kind == kCkCrc32     ? crc_finish(a.acc->crc0, a.isize, a.tab)
+                     : a.kind == kCkAdler32 ? adler_finish(a.acc->a, a.acc->b, a.isize)
+                                            : 0u;
+  container_trailer(a.kind, c, a.isize, a.out + a.hdr_len + a.body_bytes);
 }
 
 }  // namespace zb

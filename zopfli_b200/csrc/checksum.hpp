@@ -86,6 +86,21 @@ ZB_HD uint32_t adler_finish(uint64_t a, uint64_t b, uint64_t n) {
   return (uint32_t)((s2 << 16) | s1);
 }
 
+// The container trailer at tr: gzip (gzip_container.c:106-116) CRC-32 then ISIZE, both little-endian; zlib
+// (zlib_container.c:67-71) Adler-32, big-endian.  Returns its length, 0 for kCkNone.
+ZB_HD int container_trailer(int kind, uint32_t checksum, uint64_t isize, uint8_t* tr) {
+  if (kind == kCkCrc32) {
+    for (int k = 0; k < 4; k++) tr[k] = (uint8_t)(checksum >> (8 * k));
+    for (int k = 0; k < 4; k++) tr[4 + k] = (uint8_t)(isize >> (8 * k));
+    return 8;
+  }
+  if (kind == kCkAdler32) {
+    for (int k = 0; k < 4; k++) tr[k] = (uint8_t)(checksum >> (24 - 8 * k));
+    return 4;
+  }
+  return 0;
+}
+
 // where the device kernels add their slices' contributions
 struct ChecksumAcc {
   uint32_t crc0, pad;

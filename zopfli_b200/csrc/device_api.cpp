@@ -3,13 +3,12 @@
 // is emitted behind the container header in a device allocation, and the checksum is computed on the device.
 // Also the device half of the block-emission seam (ZopfliB200DeviceEmitBlocks), which needs engine calls
 // the host-only test build of api.cpp does not have.
-#include <stdio.h>
-
 #include <vector>
 
 #include "../../include/zopfli_b200.h"
 #include "api.hpp"
 #include "checksum.hpp"
+#include "dist_layout.hpp"
 #include "driver.hpp"
 #include "emit_bits.hpp"
 #include "engine.hpp"
@@ -24,12 +23,12 @@ int compress_device_to_device(const ZopfliOptions* options, ZopfliFormat fmt, co
     return 1;
   const int dev = (insize == 0 && !dev_in) ? Engine::current_device() : Engine::pointer_device(dev_in);
   if (dev < 0) return 1;
-  const double t0 = api_now_ms();
+  const double t0 = now_ms();
   const int ck = fmt == ZOPFLI_FORMAT_GZIP ? kCkCrc32 : (fmt == ZOPFLI_FORMAT_ZLIB ? kCkAdler32 : kCkNone);
   Engine::Lease eng(dev);
   eng->set_input_device_copy(dev_in, insize, stream, ck);
   std::vector<Piece> pieces;
-  deflate_units(*eng, options, 2, true, nullptr, api_master_units(insize), 0, pieces);
+  deflate_units(*eng, options, 2, true, master_blocks(0, insize), 0, pieces);
   std::vector<Engine::EmitPiece> ep;
   std::vector<uint64_t> layout;
   const uint64_t total = place_pieces(pieces, 0, 0, ep, &layout, options->verbose != 0);
@@ -38,12 +37,8 @@ int compress_device_to_device(const ZopfliOptions* options, ZopfliFormat fmt, co
   size_t n = 0;
   unsigned char* out = eng->emit_to_device(ep, total, hdr, hdr_len, ck, stream, &n);
   if (options->verbose) {  // the reports ZopfliCompress prints after the deflate body and after the container
-    const size_t deflated = (size_t)((total + 7) / 8);
-    fprintf(stderr, "Original Size: %lu, Deflate: %lu, Compression: %f%% Removed\n", (unsigned long)insize,
-            (unsigned long)deflated, 100.0 * (double)(insize - deflated) / (double)insize);
-    if (fmt != ZOPFLI_FORMAT_DEFLATE)
-      fprintf(stderr, "Original Size: %d, %s: %d, Compression: %f%% Removed\n", (int)insize,
-              fmt == ZOPFLI_FORMAT_GZIP ? "Gzip" : "Zlib", (int)n, 100.0 * (double)(insize - n) / (double)insize);
+    report_size(ZOPFLI_FORMAT_DEFLATE, insize, (size_t)((total + 7) / 8));
+    if (fmt != ZOPFLI_FORMAT_DEFLATE) report_size(fmt, insize, n);
   }
   *dev_out = out;
   *outsize = n;

@@ -158,10 +158,8 @@ void rank_deflate(Rank& rk, const ZopfliOptions* opt, int final, const unsigned 
   eng->set_input_device(d_in, d_len);  // same stream: ordered behind the copy / receive
 
   // ---- this rank's master blocks ----
-  std::vector<std::pair<size_t, size_t>> units;
-  for (size_t m = lo; m < hi; m++) units.push_back({std::min(insize, m * (size_t)kMasterBlock), std::min(insize, (m + 1) * (size_t)kMasterBlock)});
   std::vector<Piece> pieces;
-  if (!units.empty()) deflate_units(*eng, opt, 2, final != 0 && hi == nm, nullptr, units, base, pieces);
+  if (lo < hi) deflate_units(*eng, opt, 2, final != 0 && hi == nm, master_blocks(a, b), base, pieces);
 
   // ---- every rank learns every rank's stream length (for each of the 8 possible start phases: the
   // padding of stored blocks depends on it, deflate.c:643-649) ----
@@ -203,24 +201,13 @@ void rank_deflate(Rank& rk, const ZopfliOptions* opt, int final, const unsigned 
     uint8_t* hfirst = (uint8_t*)(hall + (size_t)kMetaPerRank * W);
     DCK(cudaMemcpyAsync(hfirst, d_first, (size_t)W, cudaMemcpyDeviceToHost, st));
     DCK(cudaStreamSynchronize(st));
-    // append to the caller's buffer (util.h:134-155 capacity rule); the first byte may be the caller's
-    // partially filled last byte, and the byte at every rank boundary is shared by two ranks
-    if (total_bytes) {
-      const unsigned phase = (unsigned)(start[0] & 7);
-      unsigned char keep = 0;
-      unsigned char* dst;
-      if (phase) {
-        keep = (*out)[*outsize - 1];
-        append_reserve(total_bytes - 1, out, outsize);
-        dst = *out + *outsize - total_bytes;
-      } else {
-        dst = append_reserve(total_bytes, out, outsize);
-      }
-      eng->download(d_out, dst, total_bytes);
-      dst[0] |= keep;
-      for (int q = 1; q < W; q++)
-        if (bytes_of(q)) dst[start[q] >> 3] |= hfirst[q];
-    }
+    // append to the caller's buffer; the byte at every rank boundary is shared by two ranks
+    if (total_bytes)
+      append_stream(total_bytes, (unsigned)(start[0] & 7), out, outsize, [&](unsigned char* dst) {
+        eng->download(d_out, dst, total_bytes);
+        for (int q = 1; q < W; q++)
+          if (bytes_of(q)) dst[start[q] >> 3] |= hfirst[q];
+      });
     *bp = (unsigned char)(total_bits & 7);
   } else if (local_bytes) {
     NCK(g_nccl.GroupStart());

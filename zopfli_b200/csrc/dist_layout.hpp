@@ -1,9 +1,12 @@
-// Pure arithmetic of the multi-GPU path (dist.cpp), kept apart so it can be tested without GPUs or NCCL
-// (tests/test_sharding_gloo.py drives it over gloo): which bytes a rank owns, and where every rank's bits
-// land in the one output stream.
+// Pure arithmetic of cutting an input into master blocks and of the multi-GPU path (dist.cpp), kept apart
+// so it can be tested without GPUs or NCCL (tests/test_sharding_gloo.py drives it over gloo): which bytes
+// a rank owns, and where every rank's bits land in the one output stream.
 #pragma once
 #include <stddef.h>
 #include <stdint.h>
+
+#include <utility>
+#include <vector>
 
 #include "symbols.hpp"
 
@@ -11,6 +14,17 @@ namespace zb {
 
 inline size_t dist_num_master_blocks(size_t insize) {  // deflate.c:912-924 do/while
   return insize == 0 ? 1 : (insize + kMasterBlock - 1) / kMasterBlock;
+}
+
+// The master blocks of bytes [a, b) (deflate.c:912-924): kMasterBlock bytes each from a, the last one
+// shorter.  The do/while makes an empty range one empty master block.
+inline std::vector<std::pair<size_t, size_t>> master_blocks(size_t a, size_t b) {
+  std::vector<std::pair<size_t, size_t>> u;
+  do {
+    u.push_back({a, b - a > (size_t)kMasterBlock ? a + kMasterBlock : b});
+    a = u.back().second;
+  } while (a < b);
+  return u;
 }
 
 // Rank `rank` of `world` owns the master blocks [rank*nm/world, (rank+1)*nm/world): bytes [a, b).  Its

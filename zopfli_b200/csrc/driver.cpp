@@ -1,15 +1,21 @@
 // Host driver behind ZopfliDeflate / ZopfliDeflatePart (drop-in boundary, SURVEY 8(b)).
 //
-// Reference control flow (/root/reference/src/zopfli/deflate.c:811-931) is one master block at a
-// time, one block at a time.  Here every stage is batched over ALL master blocks of the call so
-// the GPU sees every independent unit at once (SURVEY 7.2 #5, 8(e)):
+// The reference (deflate.c:811-931) runs one master block at a time, one block at a time.  Here every
+// stage is batched over many master blocks so the GPU sees every independent unit at once (SURVEY 7.2 #5,
+// 8(e)).  The master blocks of a call are cut into up to four chunk pipelines, each on its own host thread
+// and its own pair of engine lanes, running (DESIGN.md §1):
 //
-//   stage A  GPU   greedy parse of every master block              (blocksplitter.c:288-296)
-//   stage B  host  split-point search per master block, threaded   (blocksplitter.c:215-273)
-//   stage C  GPU   optimal parse of every block of every master block (deflate.c:854-869)
-//   stage D  host  second split attempt + block-type choice        (deflate.c:872-893, 747-800)
-//   stage E  GPU   fixed-tree re-parses requested by stage D        (deflate.c:771-781)
-//   stage F  host  bit emission per block (threaded) + bit-offset splice
+//   stage A  GPU       greedy parse of every master block; the stores stay on the device and become the
+//                      stores of the split service                            (blocksplitter.c:288-296)
+//   stage B  GPU+host  split search: costs priced on the device, the decisions replayed on the host
+//                      (batched_split.hpp)                          (blocksplitter.c:43-128, 195-273)
+//   stage C  GPU       optimal parse of every block; giant blocks on the even lane, the rest on the odd
+//                                                                                (deflate.c:854-869)
+//   stage D  GPU+host  block stores concatenated and priced, second split attempt, block-type choice
+//                                                                      (deflate.c:872-893, 747-800)
+//   stage E  GPU       fixed-tree re-parses requested by stage D                  (deflate.c:771-781)
+//
+// then once per call (assemble): prefix sum over the exact block sizes, one emission launch, one copy.
 #include "driver.hpp"
 
 #include <sched.h>
@@ -29,12 +35,17 @@ namespace zb {
 
 HostTimes g_host_times;
 
-namespace {
-
 double now_ms() {
   using namespace std::chrono;
   return duration<double, std::milli>(steady_clock::now().time_since_epoch()).count();
 }
+
+bool debug_on() {
+  static int v = [] { const char* e = getenv("ZOPFLI_B200_DEBUG"); return e && atoi(e) ? 1 : 0; }();
+  return v != 0;
+}
+
+namespace {
 
 std::mutex g_time_mu;
 void add_time(double& acc, double ms) {
@@ -42,10 +53,6 @@ void add_time(double& acc, double ms) {
   acc += ms;
 }
 
-bool debug_on() {
-  static int v = [] { const char* e = getenv("ZOPFLI_B200_DEBUG"); return e && atoi(e) ? 1 : 0; }();
-  return v != 0;
-}
 double g_debug_t0 = 0;
 void debug_mark(int chunk, const char* what) {
   if (debug_on()) fprintf(stderr, "[zb] %8.1f ms  chunk %d  %s\n", now_ms() - g_debug_t0, chunk, what);
@@ -101,21 +108,36 @@ void parallel_for(size_t n, F fn) {
   for (auto& t : th) t.join();
 }
 
-struct FinalBlock {
-  size_t lstart, lend;       // symbol range in the master block's store
-  size_t a, b;               // byte range (absolute input positions)
-  Engine::PlanCost c;
-  uint64_t plan;
-  bool expensive = false;
-  int fixed_req = -1;        // index into the fixed re-parse batch
-};
-
+// What the stages learn of one master block: A-B its cuts, C the size of every block's parse, D-E its pieces.
 struct Master {
   size_t ms, me;                       // byte range
-  std::vector<size_t> cuts;            // first-split block boundaries in bytes (ms, ..., me)
+  std::vector<size_t> cuts;            // block boundaries in bytes (ms, ..., me): the first split, or the second if it wins
   std::vector<uint32_t> bsize;         // symbols of every first-split block's optimal parse
   std::vector<Piece> pieces;
 };
+using BlockRef = std::pair<size_t, size_t>;  // (master block, block index)
+
+// A master block in stage D: its blocks' stores concatenated in kFin
+struct Joined {
+  uint64_t off = 0, total = 0;         // first symbol in kFin (= byte offset of the master block) and symbol count
+  std::vector<size_t> points;          // block boundaries in symbols: the first split, or the second if it wins
+  std::vector<Engine::PlanCost> cost;  // sizes of every block
+  std::vector<uint64_t> plan;          // Engine::plan_blocks handle of every block
+  uint64_t bits = 0;                   // AutoType size of the first split's blocks, summed
+  bool split2 = false;                 // the second split is attempted (deflate.c:872)
+};
+
+// A block of the final split, as AddLZ77BlockAutoType (deflate.c:747-800) weighs it
+struct FinalBlock {
+  size_t a, b;               // byte range (absolute input positions)
+  uint64_t off;              // first symbol in kFin
+  uint32_t n;                // symbols
+  Engine::PlanCost c;
+  uint64_t plan;
+  int fixed_req = -1;        // index into the fixed re-parse batch
+};
+// the fixed-tree re-parse of a block (deflate.c:771-781): its symbols in kFix and their size
+struct FixedParse { uint64_t off; uint32_t n; uint64_t bits; };
 
 // PrintBlockSplitPoints (blocksplitter.c:148-180): byte offsets of the split points from the start of the
 // store that was split (the master block), decimal then hex
@@ -135,388 +157,414 @@ uint64_t auto_type(const Engine::PlanCost& c, size_t store_size) {
   return (c.unc < fixed && c.unc < c.dyn) ? c.unc : (fixed < c.dyn ? fixed : c.dyn);
 }
 
-}  // namespace
+// AddLZ77BlockAutoType (deflate.c:747-800): the cheapest of stored, fixed and dynamic.  `fx` is the
+// block's fixed-tree re-parse, or null where none was asked for.
+Piece choose_block_type(const FinalBlock& fb, const FixedParse* fx) {
+  Piece p;
+  p.instart = fb.a;
+  p.inend = fb.b;
+  if (fb.n == 0) {  // deflate.c:763-768: the smallest empty block is a fixed one
+    p.type = 1;
+    p.nbits = 10;
+    return p;
+  }
+  const uint64_t fixedcost = fx ? fx->bits : fb.c.fixed;  // deflate.c:779
+  if (fb.c.unc < fixedcost && fb.c.unc < fb.c.dyn) {  // deflate.c:783-785
+    p.type = 0;
+  } else if (fixedcost < fb.c.dyn) {
+    p.type = 1;
+    p.nbits = fixedcost;
+    p.buf = fx ? Engine::kFix : Engine::kFin;
+    p.off = fx ? fx->off : fb.off;
+    p.n = fx ? fx->n : fb.n;
+  } else {
+    p.type = 2;
+    p.nbits = fb.c.dyn;
+    p.tree_bits = (uint32_t)fb.c.tree;
+    p.buf = Engine::kFin;
+    p.off = fb.off;
+    p.n = fb.n;
+    p.plan = fb.plan;
+  }
+  return p;
+}
 
-// in_base: absolute position of device/engine byte 0 (the engine holds bytes [in_base, ...)).
-void deflate_units(Engine& eng, const ZopfliOptions* opt, int btype, bool final_last, const unsigned char* in,
-                   const std::vector<std::pair<size_t, size_t>>& units, size_t in_base,
+// btype 0 (deflate.c:826-828): every unit one stored piece
+void deflate_stored(const std::vector<std::pair<size_t, size_t>>& units, bool final_last, std::vector<Piece>& pieces) {
+  for (size_t m = 0; m < units.size(); m++) {
+    Piece p;
+    p.type = 0;
+    p.instart = units[m].first;
+    p.inend = units[m].second;
+    p.final = final_last && m + 1 == units.size();
+    p.unit = (uint32_t)m;
+    pieces.push_back(p);
+  }
+}
+
+// btype 1 (deflate.c:829-841): one fixed-tree optimal parse per unit
+void deflate_fixed(Engine& eng, const std::vector<std::pair<size_t, size_t>>& units, size_t in_base, bool final_last,
                    std::vector<Piece>& pieces) {
   const size_t nm = units.size();
-  std::vector<Master> M(nm);
-  for (size_t m = 0; m < nm; m++) { M[m].ms = units[m].first; M[m].me = units[m].second; }
-  (void)in;
-
-  if (btype == 0) {  // deflate.c:826-828
-    for (size_t m = 0; m < nm; m++) {
-      Piece p;
-      p.type = 0;
-      p.instart = M[m].ms;
-      p.inend = M[m].me;
-      p.final = final_last && m + 1 == nm;
-      p.unit = (uint32_t)m;
-      pieces.push_back(p);
-    }
-    return;
+  std::vector<ParseRange> pr;
+  for (auto& u : units) pr.push_back({u.first - in_base, u.second - in_base, 2, 0});
+  std::vector<uint32_t> sizes;
+  std::vector<uint64_t> costs;
+  eng.parse_keep(pr, Engine::kFix, sizes, costs, 0);
+  std::vector<Engine::PlanReq> rq;
+  for (size_t m = 0; m < nm; m++) rq.push_back({pr[m].instart, sizes[m], (uint32_t)Engine::kFix});
+  std::vector<Engine::PlanCost> pc;
+  std::vector<uint64_t> ph;
+  eng.plan_blocks(rq, pc, ph, 0);
+  for (size_t m = 0; m < nm; m++) {
+    Piece p;
+    p.type = 1;
+    p.buf = Engine::kFix;
+    p.off = pr[m].instart;
+    p.n = sizes[m];
+    p.nbits = pc[m].fixed;
+    p.instart = units[m].first;
+    p.inend = units[m].second;
+    p.final = final_last && m + 1 == nm;
+    p.unit = (uint32_t)m;
+    pieces.push_back(p);
   }
-  if (btype == 1) {  // deflate.c:829-841: one fixed-tree optimal parse per unit
-    std::vector<ParseRange> pr;
-    for (auto& mb : M) pr.push_back({mb.ms - in_base, mb.me - in_base, 2, 0});
-    std::vector<uint32_t> sizes;
-    std::vector<uint64_t> costs;
-    eng.parse_keep(pr, Engine::kFix, sizes, costs, 0);
-    std::vector<Engine::PlanReq> rq;
-    for (size_t m = 0; m < nm; m++) rq.push_back({M[m].ms - in_base, sizes[m], (uint32_t)Engine::kFix});
-    std::vector<Engine::PlanCost> pc;
-    std::vector<uint64_t> ph;
-    eng.plan_blocks(rq, pc, ph, 0);
-    for (size_t m = 0; m < nm; m++) {
-      Piece p;
-      p.type = 1;
-      p.buf = Engine::kFix;
-      p.off = M[m].ms - in_base;
-      p.n = sizes[m];
-      p.nbits = pc[m].fixed;
-      p.instart = M[m].ms;
-      p.inend = M[m].me;
-      p.final = final_last && m + 1 == nm;
-      p.unit = (uint32_t)m;
-      pieces.push_back(p);
-    }
-    return;
-  }
+}
 
-  // The master blocks are processed as a few independent chunk pipelines (stages A-E each), one
-  // host thread and one pair of engine lanes per chunk: while one chunk's split search waits on
-  // round trips or its longest DP chain is still running, the others keep the GPU busy.
-  auto run_chunk = [&](const std::vector<size_t>& cm, int lane_g, int lane_r) {
-  const size_t nc = cm.size();
-  const int cid = lane_g / 2;
-  double t0 = now_ms();
-  debug_mark(cid, "start");
-  const size_t maxblocks = (size_t)opt->blocksplittingmax;
-  if (opt->blocksplitting) {
+// How a call's master blocks run: as `nchunks` chunk pipelines, each taking its master blocks in batches
+// of at most `batch`, with the blocks of `giant` bytes or more parsed on their own lane.
+struct Schedule { size_t nchunks, batch; uint64_t giant; };
+Schedule schedule(size_t nm, uint64_t device_memory) {
+  Schedule s;
+  s.nchunks = 4;
+  if (const char* e = getenv("ZOPFLI_B200_CHUNKS")) s.nchunks = (size_t)atoi(e);
+  s.nchunks = std::max<size_t>(1, std::min<size_t>(std::min<size_t>(s.nchunks, Engine::kLanes / 2), nm / 4));
+  if (nm < 8) s.nchunks = 1;
+  if (const char* e = getenv("ZOPFLI_B200_FORCE_CHUNKS")) s.nchunks = std::min<size_t>((size_t)atoi(e), std::min<size_t>(nm, Engine::kLanes / 2));  // tests
+  if (s.nchunks < 1) s.nchunks = 1;
+  // A pipeline takes its master blocks in batches because the lane arenas cost ~140 MB per master
+  // block in flight (~100 B per parse position + ~22 B per key position, two lanes).  The batch is as
+  // large as a quarter of the device memory allows (180 GB: ~80 master blocks per pipeline), so the
+  // 100 MB bench and a 134 MB shard of the 1 GiB config run as ONE wave per pipeline -- every extra
+  // wave costs a whole A + B + longest-chain latency -- and the batches of a longer input are balanced.
+  s.batch = std::max<size_t>(8, (size_t)(device_memory / 4 / ((uint64_t)s.nchunks * 140000000ull)));
+  if (const char* e = getenv("ZOPFLI_B200_BATCH")) s.batch = std::max<size_t>(1, (size_t)atoi(e));
+  s.giant = 250000;
+  if (const char* e = getenv("ZOPFLI_B200_GIANT")) s.giant = strtoull(e, nullptr, 10);  // tests: force the two-lane path
+  return s;
+}
+
+// One deflate_units call with btype 2: the engine, its options, and the master blocks.  Every stage
+// below names the fields of Master it fills; the chunk pipelines work on disjoint master blocks.
+struct Call {
+  Engine& eng;
+  const ZopfliOptions* opt;
+  size_t in_base;   // absolute position of engine byte 0
+  bool final_last;
+  uint64_t giant;
+  std::vector<Master> M;
+
+  // Stages A and B for the master blocks cm, on `lane`: their first-split cuts (M[m].cuts)
+  void first_split(const std::vector<size_t>& cm, int lane, int cid) {
+    if (!opt->blocksplitting) {
+      for (size_t m : cm) M[m].cuts = {M[m].ms, M[m].me};
+      return;
+    }
+    const double t0 = now_ms();
     // ---- stage A: greedy parse of every master block (blocksplitter.c:288-296).  The greedy stores
     // never leave the device: they become the stores of the split service, and only the byte positions
     // of the chosen split points come back (blocksplitter.c:303-313)
     std::vector<ParseRange> pr;
     for (size_t m : cm) pr.push_back({M[m].ms - in_base, M[m].me - in_base, 0, 0});
     std::vector<uint32_t> gsize;
-    eng.greedy_to_split(pr, gsize, lane_g);  // stages A and B sit on the critical path: high-priority lane
-    double t1 = now_ms();
+    eng.greedy_to_split(pr, gsize, lane);
+    const double t1 = now_ms();
     debug_mark(cid, "A greedy done");
     add_time(g_host_times.other, t1 - t0);
     // ---- stage B: split search (costs on the device, decisions on the host) ----
     std::vector<size_t> sizes(gsize.begin(), gsize.end());
     std::vector<std::vector<size_t>> lps =
-        batched_block_split(sizes, maxblocks, [&](const std::vector<EvalReq>& r, std::vector<uint64_t>& c) {
-          eng.split_eval(reinterpret_cast<const Engine::SplitReq*>(r.data()), r.size(), c.data(), lane_g);
+        batched_block_split(sizes, (size_t)opt->blocksplittingmax, [&](const std::vector<EvalReq>& r, std::vector<uint64_t>& c) {
+          eng.split_eval(reinterpret_cast<const Engine::SplitReq*>(r.data()), r.size(), c.data(), lane);
         });
     std::vector<Engine::SplitPos> want;
-    for (size_t q = 0; q < nc; q++)
+    for (size_t q = 0; q < cm.size(); q++)
       for (size_t p : lps[q]) want.push_back({(uint32_t)q, (uint32_t)p});
     std::vector<uint32_t> bytepos;
-    eng.split_positions(want, bytepos, lane_g);
+    eng.split_positions(want, bytepos, lane);
     size_t w = 0;
-    for (size_t q = 0; q < nc; q++) {
+    for (size_t q = 0; q < cm.size(); q++) {
       Master& mb = M[cm[q]];
       mb.cuts.push_back(mb.ms);
       for (size_t k = 0; k < lps[q].size(); k++) mb.cuts.push_back(mb.ms + bytepos[w++]);
       mb.cuts.push_back(mb.me);
       if (opt->verbose) print_split_points(mb.cuts, mb.ms);
     }
-    double t2 = now_ms();
     debug_mark(cid, "B split done");
-    add_time(g_host_times.split, t2 - t1);
-    t0 = t2;
-  } else {
-    for (size_t m : cm) { M[m].cuts.push_back(M[m].ms); M[m].cuts.push_back(M[m].me); }
+    add_time(g_host_times.split, now_ms() - t1);
   }
 
-  // ---- stage C: optimal parse of every block (deflate.c:854-869); the stores stay on the device ----
-  {
+  // Stage C (deflate.c:854-869) on `lane`: the optimal parse of the given blocks, kept on the device
+  // (kPack); the symbol count of each goes to M[m].bsize
+  void parse_blocks(const std::vector<BlockRef>& blocks, int lane) {
     std::vector<ParseRange> pr;
-    std::vector<std::pair<size_t, size_t>> owner;
-    for (size_t m : cm)
-      for (size_t i = 0; i + 1 < M[m].cuts.size(); i++) {
-        pr.push_back({M[m].cuts[i] - in_base, M[m].cuts[i + 1] - in_base, 1, opt->numiterations});
-        owner.push_back({m, i});
-      }
-    // The critical path of this stage is the DP chain of the largest blocks.  Giant blocks go to
-    // the even engine lane on their own (their tables are ready within milliseconds, so their iterate
-    // kernel starts at once); everything else is prepared and parsed on the odd lane meanwhile.
-    uint64_t kGiant = 250000;
-    if (const char* e = getenv("ZOPFLI_B200_GIANT")) kGiant = strtoull(e, nullptr, 10);  // tests: force the two-lane path
-    std::vector<ParseRange> prs[2];
-    std::vector<size_t> idx[2];
-    for (size_t k = 0; k < pr.size(); k++) {
-      const int lane = (pr[k].inend - pr[k].instart >= kGiant) ? 0 : 1;
-      prs[lane].push_back(pr[k]);
-      idx[lane].push_back(k);
+    for (const BlockRef& k : blocks) {
+      const std::vector<size_t>& cuts = M[k.first].cuts;
+      pr.push_back({cuts[k.second] - in_base, cuts[k.second + 1] - in_base, 1, opt->numiterations});
     }
-    for (size_t m : cm) M[m].bsize.assign(M[m].cuts.size() - 1, 0);
     const bool want_iters = opt->verbose || opt->verbose_more;
-    auto parse_lane = [&](int which, int lane) {
-      std::vector<uint32_t> sizes;
-      std::vector<uint64_t> costs, itc;
-      eng.parse_keep(prs[which], Engine::kPack, sizes, costs, lane, want_iters ? &itc : nullptr);
-      for (size_t q = 0; q < idx[which].size(); q++) {
-        const size_t k = idx[which][q];
-        M[owner[k].first].bsize[owner[k].second] = sizes[q];
-      }
-      if (want_iters && !itc.empty()) {  // squeeze.c:493-495, block after block
-        std::lock_guard<std::mutex> g(g_time_mu);
-        const size_t stride = itc.size() / idx[which].size();
-        for (size_t q = 0; q < idx[which].size(); q++) {
-          uint64_t best = ~(uint64_t)0;
-          for (size_t i = 0; i < stride && i < (size_t)opt->numiterations; i++) {
-            const uint64_t c = itc[q * stride + i];
-            if (c == ~(uint64_t)0) break;
-            if (opt->verbose_more || c < best) fprintf(stderr, "Iteration %d: %d bit\n", (int)i, (int)c);
-            if (c < best) best = c;
-          }
+    std::vector<uint32_t> sizes;
+    std::vector<uint64_t> costs, itc;
+    eng.parse_keep(pr, Engine::kPack, sizes, costs, lane, want_iters ? &itc : nullptr);
+    for (size_t q = 0; q < blocks.size(); q++) M[blocks[q].first].bsize[blocks[q].second] = sizes[q];
+    if (want_iters && !itc.empty()) {  // squeeze.c:493-495, block after block
+      std::lock_guard<std::mutex> g(g_time_mu);
+      const size_t stride = itc.size() / blocks.size();
+      for (size_t q = 0; q < blocks.size(); q++) {
+        uint64_t best = ~(uint64_t)0;
+        for (size_t i = 0; i < stride && i < (size_t)opt->numiterations; i++) {
+          const uint64_t c = itc[q * stride + i];
+          if (c == ~(uint64_t)0) break;
+          if (opt->verbose_more || c < best) fprintf(stderr, "Iteration %d: %d bit\n", (int)i, (int)c);
+          if (c < best) best = c;
         }
       }
-    };
+    }
+  }
 
-    // ---- stages D-E for a set of master blocks whose blocks are all parsed: second split attempt,
-    // block types (deflate.c:872-893, 747-800).  Works on sizes only; every store stays on the device.
-    auto finish = [&](const std::vector<size_t>& ms, int lane) {
-      const size_t nq = ms.size();
-      if (nq == 0) return;
-      double td0 = now_ms();
-      // D1: concatenate the block stores of every master block (ZopfliAppendLZ77Store, deflate.c:863)
-      std::vector<Engine::SymCopy> copies;
-      std::vector<std::vector<size_t>> first_points(nq);
-      std::vector<uint64_t> moff(nq), total(nq, 0);
-      std::vector<char> want2(nq, 0);
-      std::vector<uint64_t> soff;
-      std::vector<uint32_t> ssize;
-      std::vector<size_t> who;
-      for (size_t q = 0; q < nq; q++) {
-        const Master& mb = M[ms[q]];
-        moff[q] = mb.ms - in_base;
-        for (size_t i = 0; i < mb.bsize.size(); i++) {
-          copies.push_back({mb.cuts[i] - in_base, moff[q] + total[q], mb.bsize[i], 0});
-          total[q] += mb.bsize[i];
-          if (i + 1 < mb.bsize.size()) first_points[q].push_back((size_t)total[q]);
-        }
-        want2[q] = opt->blocksplitting && first_points[q].size() > 1;  // deflate.c:872
-        if (want2[q]) { who.push_back(q); soff.push_back(moff[q]); ssize.push_back((uint32_t)total[q]); }
+  // Stage D, first part, on `lane`: the block stores of every master block of ms concatenated in kFin
+  // (ZopfliAppendLZ77Store, deflate.c:863) and the sizes of the first split's blocks (deflate.c:862:
+  // AutoType over each block's own store)
+  std::vector<Joined> join_blocks(const std::vector<size_t>& ms, int lane) {
+    std::vector<Joined> J(ms.size());
+    std::vector<Engine::SymCopy> copies;
+    std::vector<Engine::PlanReq> rq;
+    std::vector<uint64_t> soff;
+    std::vector<uint32_t> ssize;
+    for (size_t q = 0; q < ms.size(); q++) {
+      const Master& mb = M[ms[q]];
+      Joined& j = J[q];
+      j.off = mb.ms - in_base;
+      for (size_t i = 0; i < mb.bsize.size(); i++) {
+        copies.push_back({mb.cuts[i] - in_base, j.off + j.total, mb.bsize[i], 0});
+        rq.push_back({j.off + j.total, mb.bsize[i], (uint32_t)Engine::kFin});
+        j.total += mb.bsize[i];
+        if (i + 1 < mb.bsize.size()) j.points.push_back((size_t)j.total);
       }
-      eng.concat_stores(copies, soff, ssize, lane);
-      // sizes of the first split's blocks (deflate.c:862: AutoType over each block's own store)
-      std::vector<Engine::PlanReq> rq;
-      std::vector<size_t> rq_base(nq);
-      for (size_t q = 0; q < nq; q++) {
-        const Master& mb = M[ms[q]];
-        rq_base[q] = rq.size();
-        uint64_t so = 0;
-        for (size_t i = 0; i < mb.bsize.size(); i++) { rq.push_back({moff[q] + so, mb.bsize[i], (uint32_t)Engine::kFin}); so += mb.bsize[i]; }
+      j.split2 = opt->blocksplitting && j.points.size() > 1;
+      if (j.split2) { soff.push_back(j.off); ssize.push_back((uint32_t)j.total); }
+    }
+    eng.concat_stores(copies, soff, ssize, lane);
+    std::vector<Engine::PlanCost> c;
+    std::vector<uint64_t> h;
+    eng.plan_blocks(rq, c, h, lane);
+    for (size_t q = 0, k = 0; q < ms.size(); q++)
+      for (size_t i = 0; i < M[ms[q]].bsize.size(); i++, k++) {
+        J[q].cost.push_back(c[k]);
+        J[q].plan.push_back(h[k]);
+        J[q].bits += auto_type(c[k], M[ms[q]].bsize[i]);
       }
-      std::vector<Engine::PlanCost> c1;
-      std::vector<uint64_t> h1;
-      eng.plan_blocks(rq, c1, h1, lane);
-      std::vector<uint64_t> totalcost(nq, 0);
-      for (size_t q = 0; q < nq; q++)
-        for (size_t i = 0; i < M[ms[q]].bsize.size(); i++) totalcost[q] += auto_type(c1[rq_base[q] + i], M[ms[q]].bsize[i]);
-      // D2: second split attempt on the concatenated stores (deflate.c:872-893)
-      std::vector<std::vector<size_t>> second(nq);
-      std::vector<Engine::PlanCost> c2;
-      std::vector<uint64_t> h2;
-      std::vector<size_t> rq2_base(nq, 0);
-      std::vector<char> use2(nq, 0);
-      if (!who.empty()) {
-        std::vector<size_t> sizes(ssize.begin(), ssize.end());
-        std::vector<std::vector<size_t>> r =
-            batched_block_split(sizes, maxblocks, [&](const std::vector<EvalReq>& rr, std::vector<uint64_t>& c) {
-              eng.split_eval(reinterpret_cast<const Engine::SplitReq*>(rr.data()), rr.size(), c.data(), lane);
-            });
-        std::vector<Engine::PlanReq> rq2;
-        for (size_t k = 0; k < who.size(); k++) {
-          const size_t q = who[k];
-          second[q] = r[k];
-          rq2_base[q] = rq2.size();
-          for (size_t i = 0; i <= r[k].size(); i++) {
-            const size_t a = i == 0 ? 0 : r[k][i - 1], b = i == r[k].size() ? (size_t)total[q] : r[k][i];
-            rq2.push_back({moff[q] + a, (uint32_t)(b - a), (uint32_t)Engine::kFin});
-          }
-        }
-        eng.plan_blocks(rq2, c2, h2, lane);
-        std::vector<Engine::SplitPos> want;
-        std::vector<size_t> want_base(who.size(), 0);
-        for (size_t k = 0; k < who.size(); k++) {
-          const size_t q = who[k];
-          uint64_t totalcost2 = 0;
-          for (size_t i = 0; i <= second[q].size(); i++) totalcost2 += auto_type(c2[rq2_base[q] + i], (size_t)total[q]);
-          use2[q] = totalcost2 < totalcost[q];
-          want_base[k] = want.size();
-          if (use2[q] || opt->verbose)
-            for (size_t p : second[q]) want.push_back({(uint32_t)k, (uint32_t)p});
-        }
-        // byte positions of the adopted second-pass split points (lz77->pos, deflate.c:769)
-        std::vector<uint32_t> bytepos;
-        eng.split_positions(want, bytepos, lane);
-        for (size_t k = 0; k < who.size(); k++) {
-          const size_t q = who[k];
-          if (!use2[q] && !opt->verbose) continue;
-          Master& mb = M[ms[q]];
-          std::vector<size_t> cuts2(1, mb.ms);
-          for (size_t i = 0; i < second[q].size(); i++) cuts2.push_back(mb.ms + bytepos[want_base[k] + i]);
-          cuts2.push_back(mb.me);
-          if (opt->verbose) print_split_points(cuts2, mb.ms);  // ZopfliBlockSplitLZ77 reports its points whether or not they win
-          if (use2[q]) mb.cuts.swap(cuts2);
-        }
+    return J;
+  }
+
+  // Stage D, second part (deflate.c:872-893): the second split attempt on the concatenated stores.  Where
+  // it wins, J[q] takes its points and sizes and M[ms[q]].cuts its byte boundaries.
+  void second_split(const std::vector<size_t>& ms, std::vector<Joined>& J, int lane) {
+    std::vector<size_t> who, sizes;
+    for (size_t q = 0; q < ms.size(); q++)
+      if (J[q].split2) { who.push_back(q); sizes.push_back((size_t)J[q].total); }
+    if (who.empty()) return;
+    std::vector<std::vector<size_t>> r =
+        batched_block_split(sizes, (size_t)opt->blocksplittingmax, [&](const std::vector<EvalReq>& rr, std::vector<uint64_t>& c) {
+          eng.split_eval(reinterpret_cast<const Engine::SplitReq*>(rr.data()), rr.size(), c.data(), lane);
+        });
+    std::vector<Engine::PlanReq> rq;
+    std::vector<size_t> rq_base(who.size());
+    for (size_t k = 0; k < who.size(); k++) {
+      const Joined& j = J[who[k]];
+      rq_base[k] = rq.size();
+      for (size_t i = 0; i <= r[k].size(); i++) {
+        const size_t a = i == 0 ? 0 : r[k][i - 1], b = i == r[k].size() ? (size_t)j.total : r[k][i];
+        rq.push_back({j.off + a, (uint32_t)(b - a), (uint32_t)Engine::kFin});
       }
-      // final blocks and the fixed-tree re-parses they ask for (AddLZ77BlockAutoType deflate.c:747-800)
-      std::vector<std::vector<FinalBlock>> finals(nq);
-      std::vector<ParseRange> prf;
-      for (size_t q = 0; q < nq; q++) {
-        const Master& mb = M[ms[q]];
-        const std::vector<size_t>& points = use2[q] ? second[q] : first_points[q];
-        const std::vector<Engine::PlanCost>& cc = use2[q] ? c2 : c1;
-        const std::vector<uint64_t>& hh = use2[q] ? h2 : h1;
-        const size_t base = use2[q] ? rq2_base[q] : rq_base[q];
-        for (size_t i = 0; i <= points.size(); i++) {
-          FinalBlock fb;
-          fb.lstart = i == 0 ? 0 : points[i - 1];
-          fb.lend = i == points.size() ? (size_t)total[q] : points[i];
-          fb.a = mb.cuts[i];
-          fb.b = mb.cuts[i + 1];
-          fb.c = cc[base + i];
-          fb.plan = hh[base + i];
-          fb.expensive = ((size_t)total[q] < 1000) || ((double)fb.c.fixed <= (double)fb.c.dyn * 1.1);  // :760
-          if (fb.lstart == fb.lend) fb.expensive = false;
-          if (fb.expensive) {
-            fb.fixed_req = (int)prf.size();
-            prf.push_back({fb.a - in_base, fb.b - in_base, 2, 0});
-          }
-          finals[q].push_back(fb);
+    }
+    std::vector<Engine::PlanCost> c;
+    std::vector<uint64_t> h;
+    eng.plan_blocks(rq, c, h, lane);
+    std::vector<Engine::SplitPos> want;
+    std::vector<size_t> want_base(who.size());
+    std::vector<char> use(who.size());
+    for (size_t k = 0; k < who.size(); k++) {
+      uint64_t bits = 0;
+      for (size_t i = 0; i <= r[k].size(); i++) bits += auto_type(c[rq_base[k] + i], (size_t)J[who[k]].total);
+      use[k] = bits < J[who[k]].bits;
+      want_base[k] = want.size();
+      if (use[k] || opt->verbose)
+        for (size_t p : r[k]) want.push_back({(uint32_t)k, (uint32_t)p});
+    }
+    // byte positions of the adopted second-pass split points (lz77->pos, deflate.c:769)
+    std::vector<uint32_t> bytepos;
+    eng.split_positions(want, bytepos, lane);
+    for (size_t k = 0; k < who.size(); k++) {
+      if (!use[k] && !opt->verbose) continue;
+      Master& mb = M[ms[who[k]]];
+      std::vector<size_t> cuts2(1, mb.ms);
+      for (size_t i = 0; i < r[k].size(); i++) cuts2.push_back(mb.ms + bytepos[want_base[k] + i]);
+      cuts2.push_back(mb.me);
+      if (opt->verbose) print_split_points(cuts2, mb.ms);  // ZopfliBlockSplitLZ77 reports its points whether or not they win
+      if (!use[k]) continue;
+      Joined& j = J[who[k]];
+      mb.cuts.swap(cuts2);
+      j.points = r[k];
+      j.cost.assign(c.begin() + rq_base[k], c.begin() + rq_base[k] + r[k].size() + 1);
+      j.plan.assign(h.begin() + rq_base[k], h.begin() + rq_base[k] + r[k].size() + 1);
+    }
+  }
+
+  // Stage D, third part, and stage E: the final blocks of every master block of ms, the fixed-tree
+  // re-parses they ask for (deflate.c:760, 771-781) and their types (M[m].pieces)
+  void choose_blocks(const std::vector<size_t>& ms, const std::vector<Joined>& J, int lane) {
+    std::vector<std::vector<FinalBlock>> finals(ms.size());
+    std::vector<ParseRange> prf;
+    for (size_t q = 0; q < ms.size(); q++) {
+      const Joined& j = J[q];
+      for (size_t i = 0; i <= j.points.size(); i++) {
+        const size_t ls = i == 0 ? 0 : j.points[i - 1], le = i == j.points.size() ? (size_t)j.total : j.points[i];
+        FinalBlock fb{M[ms[q]].cuts[i], M[ms[q]].cuts[i + 1], j.off + ls, (uint32_t)(le - ls), j.cost[i], j.plan[i]};
+        if (le > ls && (j.total < 1000 || (double)fb.c.fixed <= (double)fb.c.dyn * 1.1)) {  // deflate.c:760
+          fb.fixed_req = (int)prf.size();
+          prf.push_back({fb.a - in_base, fb.b - in_base, 2, 0});
         }
+        finals[q].push_back(fb);
       }
-      double td1 = now_ms();
-      add_time(g_host_times.split, td1 - td0);
-      // stage E: fixed-tree re-parses (deflate.c:771-781) and their sizes
+    }
+    std::vector<FixedParse> fixed;
+    if (!prf.empty()) {
       std::vector<uint32_t> fsize;
-      std::vector<Engine::PlanCost> c3;
-      if (!prf.empty()) {
-        std::vector<uint64_t> fcost, h3;
-        eng.parse_keep(prf, Engine::kFix, fsize, fcost, lane);
-        std::vector<Engine::PlanReq> rq3;
-        for (size_t g = 0; g < prf.size(); g++) rq3.push_back({prf[g].instart, fsize[g], (uint32_t)Engine::kFix});
-        eng.plan_blocks(rq3, c3, h3, lane);
+      std::vector<uint64_t> fcost, h;
+      eng.parse_keep(prf, Engine::kFix, fsize, fcost, lane);
+      std::vector<Engine::PlanReq> rq;
+      for (size_t g = 0; g < prf.size(); g++) rq.push_back({prf[g].instart, fsize[g], (uint32_t)Engine::kFix});
+      std::vector<Engine::PlanCost> c;
+      eng.plan_blocks(rq, c, h, lane);
+      for (size_t g = 0; g < prf.size(); g++) fixed.push_back({prf[g].instart, fsize[g], c[g].fixed});
+    }
+    for (size_t q = 0; q < ms.size(); q++)
+      for (size_t i = 0; i < finals[q].size(); i++) {
+        const FinalBlock& fb = finals[q][i];
+        Piece p = choose_block_type(fb, fb.fixed_req >= 0 ? &fixed[fb.fixed_req] : nullptr);
+        p.final = final_last && ms[q] + 1 == M.size() && i + 1 == finals[q].size();
+        p.unit = (uint32_t)ms[q];
+        M[ms[q]].pieces.push_back(p);
       }
-      for (size_t q = 0; q < nq; q++) {
-        Master& mb = M[ms[q]];
-        for (size_t i = 0; i < finals[q].size(); i++) {
-          const FinalBlock& fb = finals[q][i];
-          Piece p;
-          p.final = final_last && ms[q] + 1 == nm && i + 1 == finals[q].size();
-          p.unit = (uint32_t)ms[q];
-          p.instart = fb.a;
-          p.inend = fb.b;
-          if (fb.lstart == fb.lend) {  // deflate.c:763-768: the smallest empty block is a fixed one
-            p.type = 1;
-            p.n = 0;
-            p.nbits = 10;
-            mb.pieces.push_back(p);
-            continue;
-          }
-          const uint64_t fixedcost = fb.expensive ? c3[fb.fixed_req].fixed : fb.c.fixed;  // deflate.c:779
-          if (fb.c.unc < fixedcost && fb.c.unc < fb.c.dyn) {  // deflate.c:783-785
-            p.type = 0;
-            p.instart = fb.a;
-            p.inend = fb.b;
-          } else if (fixedcost < fb.c.dyn) {
-            p.type = 1;
-            p.nbits = fixedcost;
-            if (fb.expensive) { p.buf = Engine::kFix; p.off = fb.a - in_base; p.n = fsize[fb.fixed_req]; }
-            else { p.buf = Engine::kFin; p.off = moff[q] + fb.lstart; p.n = (uint32_t)(fb.lend - fb.lstart); }
-          } else {
-            p.type = 2;
-            p.nbits = fb.c.dyn;
-            p.tree_bits = (uint32_t)fb.c.tree;
-            p.buf = Engine::kFin;
-            p.off = moff[q] + fb.lstart;
-            p.n = (uint32_t)(fb.lend - fb.lstart);
-            p.plan = fb.plan;
-          }
-          mb.pieces.push_back(p);
-        }
-      }
-      add_time(g_host_times.other, now_ms() - td1);
-    };
+  }
 
-    if (prs[0].empty() || prs[1].empty()) {
-      const int only = prs[0].empty() ? 1 : 0;
-      parse_lane(only, lane_g);
+  // Stages D-E on `lane` for master blocks whose blocks are all parsed.  Works on sizes only; every
+  // store stays on the device.
+  void finish(const std::vector<size_t>& ms, int lane) {
+    if (ms.empty()) return;
+    const double t0 = now_ms();
+    std::vector<Joined> J = join_blocks(ms, lane);
+    second_split(ms, J, lane);
+    const double t1 = now_ms();
+    add_time(g_host_times.split, t1 - t0);
+    choose_blocks(ms, J, lane);
+    add_time(g_host_times.other, now_ms() - t1);
+  }
+
+  // D-E of the master blocks with a giant block, once the giants' parse (thread `giants`) is done
+  void finish_dirty(std::thread& giants, const std::vector<size_t>& dirty, int lane, int cid) {
+    const double tw = now_ms();
+    giants.join();
+    debug_mark(cid, "C giants parsed");
+    add_time(g_host_times.other, now_ms() - tw);
+    finish(dirty, lane);  // the giants' lane is idle now and has stream priority
+    debug_mark(cid, "D-E dirty done");
+  }
+
+  // Stages A-E of one batch of a chunk pipeline.  A, B and the giants' parse run on lane_g, the even lane,
+  // which has stream priority: they sit on the critical path.
+  void run_chunk(const std::vector<size_t>& cm, int lane_g, int lane_r) {
+    const int cid = lane_g / 2;
+    debug_mark(cid, "start");
+    first_split(cm, lane_g, cid);
+    const double t0 = now_ms();
+    // The critical path of stage C is the DP chain of the largest blocks.  Giant blocks go to the even
+    // lane on their own (their tables are ready within milliseconds, so their iterate kernel starts at
+    // once); everything else is prepared and parsed on the odd lane meanwhile.
+    std::vector<BlockRef> giants, rest;
+    for (size_t m : cm) {
+      const std::vector<size_t>& cuts = M[m].cuts;
+      M[m].bsize.assign(cuts.size() - 1, 0);
+      for (size_t i = 0; i + 1 < cuts.size(); i++) (cuts[i + 1] - cuts[i] >= giant ? giants : rest).push_back({m, i});
+    }
+    if (giants.empty() || rest.empty()) {
+      parse_blocks(giants.empty() ? rest : giants, lane_g);
       add_time(g_host_times.other, now_ms() - t0);
       finish(cm, lane_r);
-    } else {
-      std::vector<char> has_giant(nm, 0);
-      for (size_t k : idx[0]) has_giant[owner[k].first] = 1;
-      std::vector<size_t> clean, dirty;
-      for (size_t m : cm) (has_giant[m] ? dirty : clean).push_back(m);
-      std::thread tg([&] { parse_lane(0, lane_g); });
-      parse_lane(1, lane_r);
-      debug_mark(cid, "C rest parsed");
-      add_time(g_host_times.other, now_ms() - t0);
-      // A master block with a giant also has blocks on lane_r, so its D-E waits for both lanes.  The
-      // clean and the dirty D-E then run side by side, each on its own lane: their second split searches
-      // are chains of short, latency-bound rounds that leave most of the GPU idle, and when the giants end
-      // before the rest the dirty D-E no longer queues behind the clean one.  With verbose output the two
-      // run in turn, so the split-point reports keep their order (clean master blocks first).
-      auto dirty_tail = [&] {
-        double tw = now_ms();
-        tg.join();
-        debug_mark(cid, "C giants parsed");
-        add_time(g_host_times.other, now_ms() - tw);
-        finish(dirty, lane_g);  // the giants' lane is idle now and has stream priority
-        debug_mark(cid, "D-E dirty done");
-      };
-      const bool in_turn = opt->verbose || opt->verbose_more;
-      std::thread td;
-      if (!in_turn) td = std::thread(dirty_tail);
-      finish(clean, lane_r);   // overlaps the giants' DP chains still running on lane_g
-      debug_mark(cid, "D-E clean done");
-      if (in_turn) dirty_tail();
-      else td.join();
+      return;
+    }
+    std::vector<char> has_giant(M.size(), 0);
+    for (const BlockRef& k : giants) has_giant[k.first] = 1;
+    std::vector<size_t> clean, dirty;
+    for (size_t m : cm) (has_giant[m] ? dirty : clean).push_back(m);
+    std::thread tg([&] { parse_blocks(giants, lane_g); });
+    parse_blocks(rest, lane_r);
+    debug_mark(cid, "C rest parsed");
+    add_time(g_host_times.other, now_ms() - t0);
+    // A master block with a giant also has blocks on lane_r, so its D-E waits for both lanes.  The
+    // clean and the dirty D-E then run side by side, each on its own lane: their second split searches
+    // are chains of short, latency-bound rounds that leave most of the GPU idle, and when the giants end
+    // before the rest the dirty D-E no longer queues behind the clean one.  With verbose output the two
+    // run in turn, so the split-point reports keep their order (clean master blocks first).
+    const bool in_turn = opt->verbose || opt->verbose_more;
+    std::thread td;
+    if (!in_turn) td = std::thread([&] { finish_dirty(tg, dirty, lane_g, cid); });
+    finish(clean, lane_r);  // overlaps the giants' DP chains still running on lane_g
+    debug_mark(cid, "D-E clean done");
+    if (in_turn) finish_dirty(tg, dirty, lane_g, cid);
+    else td.join();
+  }
+
+  // Chunk pipeline c: its master blocks in balanced batches of at most `batch`, on lanes 2c and 2c + 1
+  void run_pipeline(const std::vector<size_t>& all, size_t batch, int c) {
+    const size_t nbatches = (all.size() + batch - 1) / batch;
+    const size_t per = nbatches ? (all.size() + nbatches - 1) / nbatches : 0;
+    for (size_t a = 0; a < all.size(); a += per) {
+      std::vector<size_t> part(all.begin() + a, all.begin() + std::min(all.size(), a + per));
+      run_chunk(part, 2 * c, 2 * c + 1);
     }
   }
-  };  // run_chunk
+};
 
-  {
-    g_debug_t0 = now_ms();
-    size_t nchunks = 4;
-    if (const char* e = getenv("ZOPFLI_B200_CHUNKS")) nchunks = (size_t)atoi(e);
-    nchunks = std::max<size_t>(1, std::min<size_t>(std::min<size_t>(nchunks, Engine::kLanes / 2), nm / 4));
-    if (nm < 8) nchunks = 1;
-    if (const char* e = getenv("ZOPFLI_B200_FORCE_CHUNKS")) nchunks = std::min<size_t>((size_t)atoi(e), std::min<size_t>(nm, Engine::kLanes / 2));  // tests
-    if (nchunks < 1) nchunks = 1;
-    std::vector<std::vector<size_t>> chunks(nchunks);
-    for (size_t m = 0; m < nm; m++) chunks[m * nchunks / nm].push_back(m);
-    // A pipeline takes its master blocks in batches because the lane arenas cost ~140 MB per master
-    // block in flight (~100 B per parse position + ~22 B per key position, two lanes).  The batch is as
-    // large as a quarter of the device memory allows (180 GB: ~80 master blocks per pipeline), so the
-    // 100 MB bench and a 134 MB shard of the 1 GiB config run as ONE wave per pipeline -- every extra
-    // wave costs a whole A + B + longest-chain latency -- and the batches of a longer input are balanced.
-    size_t batch = std::max<size_t>(8, (size_t)(eng.device_memory_total() / 4 / ((uint64_t)nchunks * 140000000ull)));
-    if (const char* e = getenv("ZOPFLI_B200_BATCH")) batch = std::max<size_t>(1, (size_t)atoi(e));
-    auto run_pipeline = [&](size_t c) {
-      const std::vector<size_t>& all = chunks[c];
-      const size_t nbatches = (all.size() + batch - 1) / batch;
-      const size_t per = nbatches ? (all.size() + nbatches - 1) / nbatches : 0;
-      for (size_t a = 0; a < all.size(); a += per) {
-        std::vector<size_t> part(all.begin() + a, all.begin() + std::min(all.size(), a + per));
-        run_chunk(part, (int)(2 * c), (int)(2 * c + 1));
-      }
-    };
-    std::vector<std::thread> th;
-    for (size_t c = 1; c < nchunks; c++) th.emplace_back([&, c] { run_pipeline(c); });
-    run_pipeline(0);
-    for (auto& t : th) t.join();
+}  // namespace
+
+void deflate_units(Engine& eng, const ZopfliOptions* opt, int btype, bool final_last,
+                   const std::vector<std::pair<size_t, size_t>>& units, size_t in_base,
+                   std::vector<Piece>& pieces) {
+  if (btype == 0) {
+    deflate_stored(units, final_last, pieces);
+    return;
   }
-  for (size_t m = 0; m < nm; m++)
-    for (auto& p : M[m].pieces) pieces.push_back(p);
+  if (btype == 1) {
+    deflate_fixed(eng, units, in_base, final_last, pieces);
+    return;
+  }
+  // The master blocks are processed as a few independent chunk pipelines (stages A-E each), one
+  // host thread and one pair of engine lanes per chunk: while one chunk's split search waits on
+  // round trips or its longest DP chain is still running, the others keep the GPU busy.
+  g_debug_t0 = now_ms();
+  const size_t nm = units.size();
+  const Schedule s = schedule(nm, eng.device_memory_total());
+  Call call{eng, opt, in_base, final_last, s.giant, std::vector<Master>(nm)};
+  for (size_t m = 0; m < nm; m++) { call.M[m].ms = units[m].first; call.M[m].me = units[m].second; }
+  std::vector<std::vector<size_t>> chunks(s.nchunks);
+  for (size_t m = 0; m < nm; m++) chunks[m * s.nchunks / nm].push_back(m);
+  std::vector<std::thread> th;
+  for (size_t c = 1; c < s.nchunks; c++) th.emplace_back([&, c] { call.run_pipeline(chunks[c], s.batch, (int)c); });
+  call.run_pipeline(chunks[0], s.batch, 0);
+  for (auto& t : th) t.join();
+  for (const Master& mb : call.M) pieces.insert(pieces.end(), mb.pieces.begin(), mb.pieces.end());
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -584,24 +632,13 @@ void assemble(Engine& eng, const std::vector<Piece>& pieces, size_t in_base, uns
   const uint64_t total = place_pieces(pieces, in_base, phase, ep, unit_bits, verbose);
   const size_t nbytes = (size_t)((total + 7) / 8);
   if (nbytes == 0) return;
-  unsigned char keep = 0;
-  unsigned char* dst;
-  if (phase) {  // the stream's first byte is the caller's last, partially filled one
-    keep = (*out)[*outsize - 1];
-    append_reserve(nbytes - 1, out, outsize);
-    dst = *out + *outsize - nbytes;
-  } else {
-    dst = append_reserve(nbytes, out, outsize);
-  }
-  eng.emit(ep, total, dst);
-  dst[0] |= keep;
+  append_stream(nbytes, phase, out, outsize, [&](unsigned char* dst) { eng.emit(ep, total, dst); });
   *bp = (unsigned char)(total & 7);
 }
 
 // ---------------------------------------------------------------------------------------------
 // splice: append position-independent span records (ZopfliB200AppendSpan) to a zopfli-style buffer
 
-// grows the buffer by n bytes under the same capacity rule and returns where they go
 unsigned char* append_reserve(size_t n, unsigned char** out, size_t* outsize) {
   size_t s = *outsize, ns = s + n;
   if (n == 0) return *out ? *out + s : nullptr;
@@ -614,17 +651,7 @@ unsigned char* append_reserve(size_t n, unsigned char** out, size_t* outsize) {
 }
 
 void append_bytes(const unsigned char* src, size_t n, unsigned char** out, size_t* outsize) {
-  if (n == 0) return;
-  size_t s = *outsize, ns = s + n;
-  size_t cap = s == 0 ? 0 : pow2_ceil(s), ncap = pow2_ceil(ns);
-  if (s == 0) {
-    *out = (unsigned char*)malloc(ncap);  // util.h:150: first append mallocs
-  } else if (ncap != cap) {
-    *out = (unsigned char*)realloc(*out, ncap);
-  }
-  if (!*out) { fprintf(stderr, "zopfli-b200: out of memory\n"); exit(EXIT_FAILURE); }
-  memcpy(*out + s, src, n);
-  *outsize = ns;
+  if (n) memcpy(append_reserve(n, out, outsize), src, n);
 }
 
 // Every piece's bit offset follows from a prefix sum over the piece sizes, so the pieces are copied
@@ -640,29 +667,11 @@ void splice_pieces(const std::vector<SpanPiece>& pieces, const unsigned char* in
   for (size_t i = 0; i < np; i++) {
     const SpanPiece& p = pieces[i];
     start[i] = pos;
-    if (!p.stored) {
-      pos += p.bits.nbits;
-    } else {  // AddNonCompressedBlock deflate.c:625-663: 3 header bits, byte align, LEN/NLEN, bytes
-      size_t q = p.instart;
-      for (;;) {
-        size_t bs = 65535;
-        if (q + bs > p.inend) bs = p.inend - q;
-        pos += 3;
-        pos = (pos + 7) & ~(uint64_t)7;
-        pos += 32 + (uint64_t)bs * 8;
-        if (q + bs >= p.inend) break;
-        q += bs;
-      }
-    }
+    pos = p.stored ? stored_end(pos, p.inend - p.instart) : pos + p.bits.nbits;
   }
   start[np] = pos;
   const size_t oldsize = *outsize, newsize = (size_t)((pos + 7) / 8);
-  if (newsize > oldsize) {  // one append of everything (util.h:134-155 capacity rule)
-    size_t cap = oldsize == 0 ? 0 : pow2_ceil(oldsize), ncap = pow2_ceil(newsize);
-    if (oldsize == 0) *out = (unsigned char*)malloc(ncap);
-    else if (ncap != cap) *out = (unsigned char*)realloc(*out, ncap);
-    if (!*out) { fprintf(stderr, "zopfli-b200: out of memory\n"); exit(EXIT_FAILURE); }
-  }
+  append_reserve(newsize - oldsize, out, outsize);  // one append of everything
   unsigned char* o = *out;
   // bytes that two pieces may share: cleared first, OR-merged after the parallel copy
   struct Edge { size_t byte; unsigned char v; };
@@ -747,7 +756,6 @@ void splice_pieces(const std::vector<SpanPiece>& pieces, const unsigned char* in
   });
   for (const Edge& e : edges)
     if (e.byte != (size_t)-1) o[e.byte] |= e.v;
-  *outsize = newsize > oldsize ? newsize : oldsize;
   *bp = (unsigned char)(pos & 7);
 }
 

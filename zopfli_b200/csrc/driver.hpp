@@ -43,9 +43,14 @@ struct SpanPiece {
 struct HostTimes { double split = 0, emit = 0, other = 0; };
 extern HostTimes g_host_times;
 
+// steady clock in milliseconds, for the stats and the ZOPFLI_B200_DEBUG timeline
+double now_ms();
+// ZOPFLI_B200_DEBUG=1: timeline of the chunk pipelines and the API calls on stderr
+bool debug_on();
+
 // Compresses the given byte ranges ("units": master blocks, or the single range of a
-// ZopfliDeflatePart call) of `in`; the engine must already hold in[in_base ...).
-void deflate_units(Engine& eng, const ZopfliOptions* opt, int btype, bool final_last, const unsigned char* in,
+// ZopfliDeflatePart call) of the input; the engine must already hold its bytes [in_base ...).
+void deflate_units(Engine& eng, const ZopfliOptions* opt, int btype, bool final_last,
                    const std::vector<std::pair<size_t, size_t>>& units, size_t in_base,
                    std::vector<Piece>& pieces);
 
@@ -66,7 +71,20 @@ uint64_t layout_pieces(const std::vector<Piece>& pieces, size_t in_base, uint64_
 void splice_pieces(const std::vector<SpanPiece>& pieces, const unsigned char* in, unsigned char* bp,
                    unsigned char** out, size_t* outsize);
 
+// Grows a zopfli-style buffer by n bytes under its capacity rule (util.h:134-155) and returns where they go.
 unsigned char* append_reserve(size_t n, unsigned char** out, size_t* outsize);
 void append_bytes(const unsigned char* src, size_t n, unsigned char** out, size_t* outsize);
+
+// Appends nbytes of stream whose first bit sits at bit `phase` of the caller's last byte (0: a fresh byte).
+// write(dst) fills all nbytes at dst; with a phase dst[0] is the caller's partly filled last byte, whose
+// bits are ORed back in afterwards.
+template <typename Write>
+void append_stream(size_t nbytes, unsigned phase, unsigned char** out, size_t* outsize, Write write) {
+  const unsigned char keep = phase ? (*out)[*outsize - 1] : 0;
+  append_reserve(phase ? nbytes - 1 : nbytes, out, outsize);
+  unsigned char* dst = *out + *outsize - nbytes;
+  write(dst);
+  dst[0] |= keep;
+}
 
 }  // namespace zb
