@@ -96,8 +96,24 @@ int ZopfliB200HostEmitBlocks(const unsigned char* in, size_t insize, const unsig
                              uint64_t* plan_val);
 /* OptimizeHuffmanForRle (deflate.c:434-518) as restated for host and device, in place, n <= 288. */
 void ZopfliB200HostOptimizeRle(uint32_t* counts, int n);
+/* The same on nhist histograms of n counts each, in place: by_segments=0 as above, 1 in the device's order
+ * (optimize_for_rle_by_segments: segment ends as a function of the segment start, reached by hops). */
+void ZopfliB200HostOptimizeRleBatch(uint32_t* counts, int n, size_t nhist, int by_segments);
 /* ZopfliLengthLimitedCodeLengths (katajainen.h:35-36) as restated for host and device. */
 int ZopfliB200HostLengthLimited(const uint32_t* freq, int n, int maxbits, unsigned* bitlengths);
+/* Tree-header bits (EncodeTree deflate.c:205-241) of nvec code-length-code count vectors clcounts[v*19 ..]:
+ * by_huffman=0 from the 7-limited package-merge, 1 from an unlimited Huffman code where it is no deeper than 7
+ * (the device's way). */
+void ZopfliB200HostTreeHeaderBits(const uint32_t* clcounts, size_t nvec, int by_huffman, uint32_t* out);
+/* The pieces of the exact dynamic block size of nhist histograms hists[h*320 ..] (taken with the end symbol's
+ * count 1, deflate.c:575): smoothed[h*320 ..] the RLE-smoothed counts (ll, then d), lengths[h*640 ..] the
+ * code lengths of the plain then the smoothed counts (320 each, distance codes patched), tree_bits[h*16 + 8*set
+ * + flags] the tree-header bits of each set under each flag combination, dyn_bits[h] the block size.  Device:
+ * the warp functions of k_split_eval / k_iterate / k_block_plan (product library only).  Host: their twins. */
+int ZopfliB200DeviceProbeParts(const uint32_t* hists, size_t nhist, uint32_t* smoothed, unsigned char* lengths,
+                               uint32_t* tree_bits, uint64_t* dyn_bits);
+int ZopfliB200HostProbeParts(const uint32_t* hists, size_t nhist, uint32_t* smoothed, unsigned char* lengths,
+                             uint32_t* tree_bits, uint64_t* dyn_bits);
 
 /* Sharding (SURVEY 8(e)): compress in[start, end) -- cut into master blocks of 1,000,000 bytes
  * counted from `start` (util.h:60; deflate.c:912-924), bytes before `start` being the LZ77

@@ -12,40 +12,52 @@ using namespace zb;
 
 __global__ void k_phases(const uint32_t* hin, unsigned long long* out, uint64_t* res) {
   __shared__ SplitSmem s;
+  __shared__ uint32_t serial[320];  // optimize_for_rle's result, for the comparison
+  __shared__ uint8_t good[320];
   const uint32_t lane = threadIdx.x;
   for (int i = lane; i < 320; i += 32) s.hist[i] = hin[i];
   __syncwarp();
   CostStage& cs = s.cs;
-  unsigned long long t[6];
+  unsigned long long t[7];
   t[0] = clock64();
-  for (int i = lane; i < 320; i += 32) cs.cnt2[i] = s.hist[i];
+  for (int i = lane; i < 320; i += 32) serial[i] = s.hist[i];
   __syncwarp();
-  if (lane < 2) optimize_for_rle(lane ? kNumD : kNumLL, cs.cnt2 + (lane ? 288 : 0), cs.good + (lane ? 288 : 0));
+  if (lane < 2) optimize_for_rle(lane ? kNumD : kNumLL, serial + (lane ? 288 : 0), good + (lane ? 288 : 0));
   __syncwarp();
   t[1] = clock64();
+  for (int i = lane; i < 320; i += 32) cs.cnt2[i] = s.hist[i];
+  __syncwarp();
+  warp_optimize_for_rle(cs.cnt2, kNumLL, cs.pm, lane);
+  warp_optimize_for_rle(cs.cnt2 + 288, kNumD, cs.pm, lane);
+  t[2] = clock64();
+  bool rle_differ = false;
+  for (int i = lane; i < 320; i += 32) rle_differ |= serial[i] != cs.cnt2[i];
+  const uint32_t rle_bad = __ballot_sync(0xffffffffu, rle_differ);
+  const unsigned long long t2b = clock64();   // the comparison stays out of the timed phases
   warp_length_limited(s.hist, kNumLL, cs.len[0], cs.pm, lane);
   warp_length_limited(s.hist + 288, kNumD, cs.len[0] + 288, cs.pm, lane);
   warp_length_limited(cs.cnt2, kNumLL, cs.len[1], cs.pm, lane);
   warp_length_limited(cs.cnt2 + 288, kNumD, cs.len[1] + 288, cs.pm, lane);
   if (lane < 2) patch_distance_codes(cs.len[lane] + 288);
   __syncwarp();
-  t[2] = clock64();
-  uint32_t walk = 0xffffffffu;  // one length at a time, one lane per (set, flags)
+  t[3] = clock64();
+  uint32_t walk = 0xffffffffu;  // one length at a time, one lane per (set, flags), package-merge per lane
   if (lane < 16) {
     const uint8_t* l = cs.len[lane >> 3];
     walk = encode_tree_size(l, l + 288, (lane & 1) != 0, (lane & 2) != 0, (lane & 4) != 0);
   }
   __syncwarp();
-  t[3] = clock64();
+  t[4] = clock64();
   const uint32_t runs = warp_tree_sizes(cs, lane);
   __syncwarp();
-  t[4] = clock64();
-  const uint64_t r = warp_dynamic_bits(s.hist, s.cs, lane);
   t[5] = clock64();
+  const uint64_t r = warp_dynamic_bits(s.hist, s.cs, lane);
+  t[6] = clock64();
   const uint32_t differ = __ballot_sync(0xffffffffu, lane < 16 && walk != runs);
   if (lane == 0) {
-    for (int i = 0; i < 5; i++) out[i] = t[i + 1] - t[i];
-    out[5] = differ;
+    for (int i = 0; i < 6; i++) out[i] = t[i + 1] - (i == 2 ? t2b : t[i]);
+    out[6] = differ;
+    out[7] = rle_bad;
     res[0] = r;
   }
 }
@@ -77,15 +89,16 @@ int main() {
   unsigned long long* dout;
   uint64_t* dres;
   cudaMalloc(&dh, 320 * 4);
-  cudaMalloc(&dout, 64);
+  cudaMalloc(&dout, 128);
   cudaMalloc(&dres, 1 << 20);
   cudaMemcpy(dh, h.data(), 320 * 4, cudaMemcpyHostToDevice);
   for (int k = 0; k < 3; k++) {
     k_phases<<<1, 32>>>(dh, dout, dres);
-    unsigned long long o[6];
+    unsigned long long o[8];
     cudaMemcpy(o, dout, sizeof(o), cudaMemcpyDeviceToHost);
-    printf("cycles: RLE smoothing %llu, 4 package merges %llu, tree sizes walked %llu, by runs %llu (%s); "
-           "warp_dynamic_bits %llu\n", o[0], o[1], o[2], o[3], o[5] ? "DIFFER" : "equal", o[4]);
+    printf("cycles: RLE smoothing serial %llu, by the warp %llu (%s); 4 package merges %llu; tree sizes walked %llu, "
+           "by runs %llu (%s); warp_dynamic_bits %llu\n", o[0], o[1], o[7] ? "DIFFER" : "equal", o[2], o[3], o[4],
+           o[6] ? "DIFFER" : "equal", o[5]);
   }
   cudaFuncSetAttribute(k_many, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
   cudaEvent_t a, b;

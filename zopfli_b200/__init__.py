@@ -51,6 +51,7 @@ EXPORTS = ["ZopfliInitOptions", "ZopfliCompress", "ZopfliDeflate", "ZopfliDeflat
            "ZopfliGzipCompress", "ZopfliZlibCompress", "ZopfliB200LZ77", "ZopfliB200LZ77Batch",
            "ZopfliB200MatchTable", "ZopfliB200DynamicBlockBits", "ZopfliB200DeviceAutoTypeBits", "ZopfliB200HostBlockSplitLZ77",
            "ZopfliB200HostBatchedSplit", "ZopfliB200HostBlockSize", "ZopfliB200HostEmitBlock", "ZopfliB200DeviceEmitBlocks", "ZopfliB200HostEmitBlocks", "ZopfliB200HostLengthLimited", "ZopfliB200HostOptimizeRle",
+           "ZopfliB200HostOptimizeRleBatch", "ZopfliB200HostTreeHeaderBits", "ZopfliB200HostProbeParts", "ZopfliB200DeviceProbeParts",
            "ZopfliB200DeflateSpan", "ZopfliB200AppendSpan", "ZopfliB200LastMasterBitOffsets", "ZopfliB200Crc32", "ZopfliB200Crc32Combine", "ZopfliB200Adler32", "ZopfliB200CompressDevice",
            "ZopfliB200DistUniqueId", "ZopfliB200DistInit", "ZopfliB200DistCompress", "ZopfliB200DistFinalize", "ZopfliB200DistShard", "ZopfliB200DistPlacement",
            "ZopfliB200GetStats", "ZopfliB200ResetStats", "ZopfliB200SetStream", "ZopfliB200Device",
@@ -178,6 +179,12 @@ class Library:
         L.ZopfliB200HostLengthLimited.argtypes = [vp, C.c_int, C.c_int, vp]
         L.ZopfliB200HostOptimizeRle.argtypes = [vp, C.c_int]
         L.ZopfliB200HostOptimizeRle.restype = None
+        L.ZopfliB200HostOptimizeRleBatch.argtypes = [vp, C.c_int, sz, C.c_int]
+        L.ZopfliB200HostOptimizeRleBatch.restype = None
+        L.ZopfliB200HostTreeHeaderBits.argtypes = [vp, sz, C.c_int, vp]
+        L.ZopfliB200HostTreeHeaderBits.restype = None
+        L.ZopfliB200HostProbeParts.argtypes = [vp, sz, vp, vp, vp, vp]
+        L.ZopfliB200HostProbeParts.restype = C.c_int
         L.ZopfliB200DeflateSpan.argtypes = [C.POINTER(ZopfliOptions), vp, sz, vp, sz, sz, C.c_int,
                                             C.POINTER(vp), C.POINTER(sz)]
         L.ZopfliB200AppendSpan.argtypes = [vp, sz, C.POINTER(C.c_ubyte), C.POINTER(vp), C.POINTER(sz)]
@@ -200,7 +207,8 @@ class Library:
                                 ("ZopfliB200Crc32Device", [vp, sz, vp, C.POINTER(C.c_uint32)], C.c_int),
                                 ("ZopfliB200Adler32Device", [vp, sz, vp, C.POINTER(C.c_uint32)], C.c_int),
                                 ("ZopfliB200DeviceEmitBlocks", [vp, sz, vp, vp, sz, sz, vp, vp, vp, vp, C.c_uint, vp, sz, vp, vp,
-                                                                vp], C.c_int)):
+                                                                vp], C.c_int),
+                                ("ZopfliB200DeviceProbeParts", [vp, sz, vp, vp, vp, vp], C.c_int)):
             f = getattr(L, name, None)
             if f is not None:
                 f.argtypes, f.restype = args, res
@@ -397,6 +405,34 @@ class Library:
         c = np.ascontiguousarray(counts, np.uint32).copy()
         self.lib.ZopfliB200HostOptimizeRle(c.ctypes.data, len(c))
         return c
+
+    def optimize_rle_batch(self, counts, by_segments):
+        """OptimizeHuffmanForRle on every row of `counts` (nhist x n): by_segments=False the host twin,
+        True the device's order (optimize_for_rle_by_segments)"""
+        c = np.ascontiguousarray(counts, np.uint32).copy()
+        self.lib.ZopfliB200HostOptimizeRleBatch(c.ctypes.data, c.shape[1], c.shape[0], 1 if by_segments else 0)
+        return c
+
+    def tree_header_bits(self, clcounts, by_huffman):
+        """tree-header bits of every row of `clcounts` (nvec x 19)"""
+        c = np.ascontiguousarray(clcounts, np.uint32)
+        out = np.zeros(len(c), np.uint32)
+        self.lib.ZopfliB200HostTreeHeaderBits(c.ctypes.data, len(c), 1 if by_huffman else 0, out.ctypes.data)
+        return out
+
+    def probe_parts(self, hists, device):
+        """the pieces of the exact dynamic block size of every row of `hists` (nhist x 320): smoothed counts,
+        code lengths (nhist x 2 x 320), tree-header bits (nhist x 2 x 8) and the size, on the device or by the
+        host twins"""
+        h = np.ascontiguousarray(hists, np.uint32)
+        n = len(h)
+        sm = np.zeros((n, 320), np.uint32)
+        ln = np.zeros((n, 2, 320), np.uint8)
+        tb = np.zeros((n, 2, 8), np.uint32)
+        dyn = np.zeros(n, np.uint64)
+        fn = self.lib.ZopfliB200DeviceProbeParts if device else self.lib.ZopfliB200HostProbeParts
+        fn(h.ctypes.data, n, sm.ctypes.data, ln.ctypes.data, tb.ctypes.data, dyn.ctypes.data)
+        return sm, ln, tb, dyn
 
     def host_length_limited(self, freq, maxbits):
         f = np.ascontiguousarray(freq, np.uint32)

@@ -615,6 +615,48 @@ void ZopfliB200HostOptimizeRle(uint32_t* counts, int n) {
   optimize_for_rle(n, counts, good);
 }
 
+void ZopfliB200HostOptimizeRleBatch(uint32_t* counts, int n, size_t nhist, int by_segments) {
+  if (n < 0 || n > kNumLL) return;
+  uint8_t good[kNumLL];
+  for (size_t h = 0; h < nhist; h++) {
+    if (by_segments) optimize_for_rle_by_segments(n, counts + h * n, good);
+    else optimize_for_rle(n, counts + h * n, good);
+  }
+}
+
+void ZopfliB200HostTreeHeaderBits(const uint32_t* clcounts, size_t nvec, int by_huffman, uint32_t* out) {
+  for (size_t v = 0; v < nvec; v++)
+    out[v] = by_huffman ? tree_header_bits_huffman(clcounts + v * 19) : tree_header_bits(clcounts + v * 19);
+}
+
+int ZopfliB200HostProbeParts(const uint32_t* hists, size_t nhist, uint32_t* smoothed, unsigned char* lengths,
+                             uint32_t* tree_bits, uint64_t* dyn_bits) {
+  static thread_local PmScratch<kNumLL, 15> pm;
+  static thread_local DynScratch ds;
+  uint8_t good[kNumLL];
+  for (size_t h = 0; h < nhist; h++) {
+    uint32_t* sm = smoothed + h * 320;
+    unsigned char* len = lengths + h * 640;
+    uint32_t hist[320];
+    memcpy(hist, hists + h * 320, sizeof(hist));
+    hist[256] = 1;  // deflate.c:575
+    memcpy(sm, hist, sizeof(hist));
+    optimize_for_rle(kNumLL, sm, good);
+    optimize_for_rle(kNumD, sm + 288, good);
+    for (int set = 0; set < 2; set++) {
+      const uint32_t* c = set ? sm : hist;
+      unsigned char* l = len + set * 320;
+      length_limited<kNumLL, 15>(c, kNumLL, 15, l, pm);
+      length_limited<kNumLL, 15>(c + 288, kNumD, 15, l + 288, pm);
+      patch_distance_codes(l + 288);
+      for (int f = 0; f < 8; f++)
+        tree_bits[h * 16 + set * 8 + f] = encode_tree_size(l, l + 288, (f & 1) != 0, (f & 2) != 0, (f & 4) != 0);
+    }
+    dyn_bits[h] = dynamic_block_bits(hist, nullptr, nullptr, ds);
+  }
+  return 0;
+}
+
 void ZopfliB200GetStats(ZopfliB200Stats* o) {
   EngineStats e = Engine::stats_all();
   o->ms_same = e.ms_same; o->ms_keys = e.ms_keys; o->ms_scan = e.ms_scan; o->ms_scatter = e.ms_scatter;

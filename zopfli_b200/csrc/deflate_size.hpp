@@ -184,18 +184,68 @@ ZB_HD unsigned clcl_rank_symbol(unsigned k) {  // RFC1951 3.2.7 transmission ord
   return (k & 1) ? 7 - h : 8 + h;
 }
 
+// Bits of the tree header given the code-length-code counts and clcode_bits = sum of clcl[i] * clcounts[i]
+// over their 7-limited code: HCLEN, the code-length code itself, the tokens and their extra bits
+ZB_HD uint32_t tree_header_bits_from(const uint32_t* clcounts, uint32_t clcode_bits) {
+  unsigned hclen = 15;
+  while (hclen > 0 && clcounts[clcl_rank_symbol(hclen + 3)] == 0) hclen--;
+  return 14 + (hclen + 4) * 3 + clcode_bits + clcounts[16] * 2 + clcounts[17] * 3 + clcounts[18] * 7;
+}
+
 // The rest of EncodeTree(size_only) once the code-length-code counts are known (deflate.c:205-241):
 // their length-limited code, HCLEN, and the bits of the header
 ZB_HD uint32_t tree_header_bits(const uint32_t* clcounts) {
   uint8_t clcl[19];
   PmScratch<19, 7> s;
   length_limited<19, 7>(clcounts, 19, 7, clcl, s);
-  unsigned hclen = 15;
-  while (hclen > 0 && clcounts[clcl_rank_symbol(hclen + 3)] == 0) hclen--;
-  uint32_t r = 14 + (hclen + 4) * 3;
+  uint32_t r = 0;
   for (int i = 0; i < 19; i++) r += clcl[i] * clcounts[i];
-  r += clcounts[16] * 2 + clcounts[17] * 3 + clcounts[18] * 7;
-  return r;
+  return tree_header_bits_from(clcounts, r);
+}
+
+// The header uses the code-length code only through sum(clcl[i] * clcounts[i]), and every optimal 7-limited
+// code has the same sum, so an unconstrained Huffman code no deeper than 7 gives it too.  Builds one in
+// registers (19 keys weight << 10 | height << 5 | slot; the lowest height wins among equal weights, which
+// keeps the tree shallow) and returns false when it comes out deeper than 7: the caller then takes the
+// package-merge (length_limited), which is exact in every case.  0, 1 or 2 used symbols get length 1 each
+// (katajainen.c:208-222).  The counts must sum to less than 2^22 (a header has at most 320 tokens).
+ZB_HD bool clcode_bits_unlimited(const uint32_t* clcounts, uint32_t* clcode_bits) {
+  const uint32_t kNone = 0xffffffffu;
+  uint32_t k[19];
+  uint32_t ns = 0, total = 0;
+ZB_UNROLL
+  for (int i = 0; i < 19; i++) {
+    const uint32_t c = clcounts[i];
+    k[i] = c ? (c << 10) | (uint32_t)i : kNone;
+    ns += c ? 1u : 0u;
+    total += c;
+  }
+  if (ns <= 2) { *clcode_bits = total; return true; }
+  uint32_t bits = 0, height = 0;
+  for (uint32_t m = 1; m < ns; m++) {
+    uint32_t m1 = kNone, m2 = kNone;
+ZB_UNROLL
+    for (int i = 0; i < 19; i++) m1 = k[i] < m1 ? k[i] : m1;
+ZB_UNROLL
+    for (int i = 0; i < 19; i++) k[i] = k[i] == m1 ? kNone : k[i];
+ZB_UNROLL
+    for (int i = 0; i < 19; i++) m2 = k[i] < m2 ? k[i] : m2;
+    const uint32_t w = (m1 >> 10) + (m2 >> 10), h1 = (m1 >> 5) & 31u, h2 = (m2 >> 5) & 31u;
+    height = (h1 > h2 ? h1 : h2) + 1;
+    const uint32_t merged = (w << 10) | (height << 5) | (m2 & 31u);
+ZB_UNROLL
+    for (int i = 0; i < 19; i++) k[i] = k[i] == m2 ? merged : k[i];
+    bits += w;   // every leaf under the new node is one bit deeper
+  }
+  *clcode_bits = bits;
+  return height <= 7;
+}
+
+// tree_header_bits by clcode_bits_unlimited where its tree fits in 7 bits (the device's way, CPU-testable)
+ZB_HD uint32_t tree_header_bits_huffman(const uint32_t* clcounts) {
+  uint32_t bits;
+  if (clcode_bits_unlimited(clcounts, &bits)) return tree_header_bits_from(clcounts, bits);
+  return tree_header_bits(clcounts);
 }
 
 // EncodeTree with out == NULL (deflate.c:105-249): bits of the tree header for one flag choice
@@ -305,6 +355,63 @@ ZB_HD void optimize_for_rle(int length, CntT* counts, uint8_t* good) {
       for (int k = a; k < b; k++) counts[k] = (CntT)mean;
     }
     limit = ahead(b);
+    a = b;
+  }
+}
+
+// Pass 3 of optimize_for_rle as a function of the segment start.  Pass 3 reads only original counts (a
+// segment is flattened after the next limit has been read from the counts at and after its end), and a
+// segment that starts at a > 0 always has limit ahead(a); only a = 0 takes counts[0] when position 0 is
+// not pinned.  So where the segment that starts at `a` ends is a pure function of a: the device evaluates
+// it with one ballot per 32 positions and hops from start to start (warp_optimize_for_rle, iterate.cuh).
+// The limit never exceeds the largest count, so it fits the count type.
+template <typename CntT>
+ZB_HD uint32_t rle_segment_limit(const CntT* counts, int length, bool good0, int a) {
+  if (a == 0 && !good0) return (uint32_t)counts[0];
+  if (a < length - 3) return (uint32_t)(((uint64_t)counts[a] + counts[a + 1] + counts[a + 2] + counts[a + 3] + 2) / 4);
+  return a < length ? (uint32_t)counts[a] : 0u;
+}
+ZB_HD bool rle_extends(uint32_t c, uint32_t limit) { return (c > limit ? c - limit : limit - c) < 4; }
+template <typename CntT>
+ZB_HD int rle_segment_end(const CntT* counts, const uint8_t* good, int length, int a) {
+  const uint32_t limit = rle_segment_limit(counts, length, good[0] != 0, a);
+  int b = a + 1;
+  while (b < length && !good[b] && rle_extends((uint32_t)counts[b], limit)) b++;
+  return b;
+}
+// whether a finished segment of `stride` counts summing to `sum` is flattened, and to what value
+ZB_HD bool rle_flatten(uint64_t sum, int stride, uint32_t* mean) {
+  if (stride < 3 || (stride == 3 && sum != 0)) return false;
+  uint64_t m = (sum + (uint64_t)(stride / 2)) / (uint64_t)stride;
+  if (m < 1) m = 1;
+  if (sum == 0) m = 0;
+  *mean = (uint32_t)m;
+  return true;
+}
+
+// optimize_for_rle in the device's order (CPU model of warp_optimize_for_rle): pinned runs, then every
+// segment start found by hopping through rle_segment_end, then each segment flattened.  `good` is caller
+// scratch of `length` bytes; length <= 288.
+template <typename CntT>
+ZB_HD void optimize_for_rle_by_segments(int length, CntT* counts, uint8_t* good) {
+  while (length > 0 && counts[length - 1] == 0) length--;
+  if (length == 0) return;
+  for (int a = 0; a < length;) {
+    int b = a + 1;
+    while (b < length && counts[b] == counts[a]) b++;
+    for (int k = a; k < b; k++) good[k] = (b - a) >= (counts[a] == 0 ? 5 : 7) ? 1 : 0;
+    a = b;
+  }
+  uint32_t starts[(288 + 31) / 32] = {0};
+  for (int a = 0; a < length; a = rle_segment_end(counts, good, length, a)) starts[a >> 5] |= 1u << (a & 31);
+  for (int a = 0; a < length;) {
+    int b = a + 1;
+    while (b < length && !((starts[b >> 5] >> (b & 31)) & 1u)) b++;
+    uint64_t sum = 0;
+    for (int k = a; k < b; k++) sum += counts[k];
+    uint32_t mean;
+    if (rle_flatten(sum, b - a, &mean))
+      for (int k = a; k < b; k++) counts[k] = (CntT)mean;
     a = b;
   }
 }

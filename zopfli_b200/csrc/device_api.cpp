@@ -75,6 +75,13 @@ int ZopfliB200Adler32Device(const unsigned char* dev_in, size_t size, void* cuda
   return device_checksum(dev_in, size, cuda_stream, kCkAdler32, adler);
 }
 
+int ZopfliB200DeviceProbeParts(const uint32_t* hists, size_t nhist, uint32_t* smoothed, unsigned char* lengths,
+                               uint32_t* tree_bits, uint64_t* dyn_bits) {
+  Engine::Lease eng;
+  eng->device_probe_parts(hists, nhist, smoothed, lengths, tree_bits, dyn_bits);
+  return 0;
+}
+
 int ZopfliB200DeviceEmitBlocks(const unsigned char* in, size_t insize, const unsigned short* litlens,
                                const unsigned short* dists, size_t n, size_t npieces, const size_t* lstart,
                                const size_t* lend, const int* btype, const int* final, unsigned bp0,

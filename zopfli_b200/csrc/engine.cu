@@ -61,6 +61,39 @@ __global__ void k_test_block_bits(Batch b, const uint32_t* hist, uint64_t* out) 
   if (lane == 0) *out = r;
 }
 
+// the pieces of warp_dynamic_bits for one histogram per CTA (ZopfliB200DeviceProbeParts)
+__global__ void k_test_probe_parts(const uint32_t* hists, uint32_t* smoothed, uint8_t* lengths, uint32_t* tree_bits,
+                                   uint64_t* dyn) {
+  __shared__ SplitSmem s;
+  const uint32_t lane = threadIdx.x, h = blockIdx.x;
+  CostStage& cs = s.cs;
+  for (int i = lane; i < 320; i += 32) s.hist[i] = hists[h * 320 + i];
+  __syncwarp();
+  if (lane == 0) s.hist[256] = 1;
+  __syncwarp();
+  for (int i = lane; i < 320; i += 32) cs.cnt2[i] = s.hist[i];
+  __syncwarp();
+  warp_optimize_for_rle(cs.cnt2, kNumLL, cs.pm, lane);
+  warp_optimize_for_rle(cs.cnt2 + 288, kNumD, cs.pm, lane);
+  warp_length_limited(s.hist, kNumLL, cs.len[0], cs.pm, lane);
+  warp_length_limited(s.hist + 288, kNumD, cs.len[0] + 288, cs.pm, lane);
+  warp_length_limited(cs.cnt2, kNumLL, cs.len[1], cs.pm, lane);
+  warp_length_limited(cs.cnt2 + 288, kNumD, cs.len[1] + 288, cs.pm, lane);
+  if (lane < 2) patch_distance_codes(cs.len[lane] + 288);
+  __syncwarp();
+  for (int i = lane; i < 320; i += 32) {
+    smoothed[h * 320 + i] = cs.cnt2[i];
+    lengths[h * 640 + i] = cs.len[0][i];
+    lengths[h * 640 + 320 + i] = cs.len[1][i];
+  }
+  __syncwarp();
+  const uint32_t t = warp_tree_sizes(cs, lane);   // overwrites cs.cnt2
+  if (lane < 16) tree_bits[h * 16 + lane] = t;
+  __syncwarp();
+  const uint64_t r = warp_dynamic_bits(s.hist, cs, lane);
+  if (lane == 0) dyn[h] = r;
+}
+
 struct Timer {
   cudaEvent_t a, b;
   Timer() { CK(cudaEventCreate(&a)); CK(cudaEventCreate(&b)); }
@@ -1361,6 +1394,31 @@ uint64_t Engine::device_block_bits(const uint32_t* hist320) {
   CK(cudaMemcpyAsync(&r, dout, 8, cudaMemcpyDeviceToHost, l.stream));
   l.sync();
   return r;
+}
+
+void Engine::device_probe_parts(const uint32_t* hists, size_t n, uint32_t* smoothed, uint8_t* lengths,
+                                uint32_t* tree_bits, uint64_t* dyn) {
+  if (n == 0) return;
+  Impl& m = *p_;
+  Lane& l = m.lane[0];
+  std::lock_guard<std::mutex> g(l.mu);
+  CK(cudaSetDevice(m.dev));
+  const size_t in_b = n * 320 * 4, sm_b = n * 320 * 4, len_b = n * 640, tb_b = n * 16 * 4, dyn_b = n * 8;
+  l.misc.ensure(dyn_b + in_b + sm_b + tb_b + len_b);
+  uint8_t* base = (uint8_t*)l.misc.p;   // 8-byte fields first, bytes last
+  uint64_t* d_dyn = (uint64_t*)base;
+  uint32_t* d_in = (uint32_t*)(base + dyn_b);
+  uint32_t* d_sm = (uint32_t*)(base + dyn_b + in_b);
+  uint32_t* d_tb = (uint32_t*)(base + dyn_b + in_b + sm_b);
+  uint8_t* d_len = base + dyn_b + in_b + sm_b + tb_b;
+  CK(cudaMemcpyAsync(d_in, hists, in_b, cudaMemcpyHostToDevice, l.stream));
+  k_test_probe_parts<<<(unsigned)n, 32, 0, l.stream>>>(d_in, d_sm, d_len, d_tb, d_dyn);
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(smoothed, d_sm, sm_b, cudaMemcpyDeviceToHost, l.stream));
+  CK(cudaMemcpyAsync(lengths, d_len, len_b, cudaMemcpyDeviceToHost, l.stream));
+  CK(cudaMemcpyAsync(tree_bits, d_tb, tb_b, cudaMemcpyDeviceToHost, l.stream));
+  CK(cudaMemcpyAsync(dyn, d_dyn, dyn_b, cudaMemcpyDeviceToHost, l.stream));
+  l.sync();
 }
 
 }  // namespace zb

@@ -85,6 +85,9 @@ class Engine {
                    std::vector<uint16_t>& same, std::vector<uint16_t>& hv, std::vector<uint16_t>& hv2);
   // test seam: device-side exact dynamic block size of a 320-bin histogram
   uint64_t device_block_bits(const uint32_t* hist320);
+  // test seam: the pieces of that size for n histograms (ZopfliB200DeviceProbeParts)
+  void device_probe_parts(const uint32_t* hists, size_t n, uint32_t* smoothed, uint8_t* lengths, uint32_t* tree_bits,
+                          uint64_t* dyn);
 
   // Split-cost service (ZopfliCalculateBlockSizeAutoType over symbol ranges, deflate.c:610-621):
   // split_begin uploads n stores given as flat symbol arrays with per-store offset/size,

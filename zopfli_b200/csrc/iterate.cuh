@@ -99,7 +99,6 @@ struct WarpPm {                        // warp-wide package-merge working set (w
 struct CostStage {                     // block-size working set
   uint32_t cnt2[320];                  // RLE-smoothed copies (ll: [0,288), d: [288,320))
   uint8_t len[2][320];                 // code lengths: set 0 plain, set 1 smoothed
-  uint8_t good[320];                   // OptimizeHuffmanForRle marks
   WarpPm pm;
 };
 struct IterSmem {
@@ -401,7 +400,7 @@ struct DynChoice { uint32_t set, flags, tree_bits; };
 // each set spread over the warp, instead of 16 lanes walking the sequence one length at a time down
 // eight diverging paths.  The counts, and so the sizes, are those encode_tree_size computes.
 __device__ __noinline__ uint32_t warp_tree_sizes(CostStage& cs, uint32_t lane) {
-  uint32_t* cl = &cs.pm.row[0][0];   // [set][flags][19] counts; the package-merge rows are free by now
+  uint32_t* cl = cs.cnt2;            // [set][flags][19] counts; the smoothed counts are spent by now
   uint32_t* starts = cs.pm.mask[0];  // run starts of one set, a bit per position
   for (int i = lane; i < 2 * 8 * 19; i += 32) cl[i] = 0;
   for (int set = 0; set < 2; set++) {
@@ -434,16 +433,120 @@ __device__ __noinline__ uint32_t warp_tree_sizes(CostStage& cs, uint32_t lane) {
     }
   }
   __syncwarp();
-  return lane < 16 ? tree_header_bits(cl + lane * 19) : 0xffffffffu;
+  // the code-length code's cost from a Huffman tree in registers; the lanes where that tree is deeper than
+  // 7 bits take the package-merge, each on its own scratch in the package-merge working set (free by now).
+  // tree_header_bits_huffman is the CPU model.
+  static_assert(16 * sizeof(PmScratch<19, 7>) + 16 * 19 <= sizeof(WarpPm), "cl-code scratch");
+  uint32_t r = 0xffffffffu, bits = 0;
+  const bool fits = lane < 16 && clcode_bits_unlimited(cl + lane * 19, &bits);
+  if (fits) r = tree_header_bits_from(cl + lane * 19, bits);
+  if (lane < 16 && !fits) {
+    PmScratch<19, 7>* pms = reinterpret_cast<PmScratch<19, 7>*>(cs.pm.key);
+    uint8_t* clcl = reinterpret_cast<uint8_t*>(pms + 16) + lane * 19;
+    length_limited<19, 7>(cl + lane * 19, 19, 7, clcl, pms[lane]);
+    bits = 0;
+    for (int i = 0; i < 19; i++) bits += clcl[i] * cl[lane * 19 + i];
+    r = tree_header_bits_from(cl + lane * 19, bits);
+  }
+  __syncwarp();
+  return r;
+}
+
+// first marked position after i in the bit words[0 .. nw) (a bit per position), or `none`
+__device__ __forceinline__ int next_mark(const uint32_t* words, int nw, int i, int none) {
+  const uint32_t b = i & 31;
+  int w = i >> 5;
+  uint32_t m = b == 31 ? 0u : words[w] & ~((2u << b) - 1u);
+  while (!m && ++w < nw) m = words[w];
+  return m ? w * 32 + (__ffs(m) - 1) : none;
+}
+
+// OptimizeHuffmanForRle (optimize_for_rle, deflate.c:434-518) by the whole warp, in place on n <= 288
+// counts in shared memory; the package-merge working set is its scratch.  Pass 1: the last non-zero count
+// by ballot.  Pass 2: run starts by ballot; each lane measures the runs that start on its positions and
+// pins the long ones, a bit per position.  Pass 3 (rle_segment_end in deflate_size.hpp): from each segment
+// start reached, the warp tests the next 32 positions against the start's limit with one ballot, so the
+// serial part is one hop per segment; then the lanes the segment starts fall on flatten them.
+// optimize_for_rle_by_segments is the CPU model of this order.
+__device__ __noinline__ void warp_optimize_for_rle(uint32_t* counts, int n, WarpPm& pm, uint32_t lane) {
+  const uint32_t full = 0xffffffffu;
+  uint32_t* ends = pm.row[0];    // end of the segment that would start at each position (0: not measured)
+  uint32_t* runs = pm.mask[0];   // run starts
+  uint32_t* pin = pm.mask[1];    // pinned positions (good_for_rle)
+  uint32_t* seg = pm.mask[2];    // segment starts
+  int length = 0;
+  for (int base = 0; base < n; base += 32) {
+    const int i = base + (int)lane;
+    const uint32_t m = __ballot_sync(full, i < n && counts[i] != 0);
+    if (m) length = base + 32 - __clz(m);
+  }
+  if (length == 0) return;
+  const int nw = (length + 31) >> 5;
+  for (int w = 0; w < nw; w++) {
+    const int i = w * 32 + (int)lane;
+    const uint32_t m = __ballot_sync(full, i < length && (i == 0 || counts[i] != counts[i - 1]));
+    if (lane == 0) runs[w] = m;
+    if ((int)lane == w) pin[w] = 0;
+  }
+  __syncwarp();
+  for (int i = lane; i < length; i += 32) {
+    if (!((runs[i >> 5] >> (i & 31)) & 1u)) continue;
+    const int end = next_mark(runs, nw, i, length);
+    if (end - i < (counts[i] == 0 ? 5 : 7)) continue;
+    for (int w = i >> 5; w <= (end - 1) >> 5; w++) {
+      const int lo = (i > w * 32 ? i : w * 32) - w * 32, hi = (end < w * 32 + 32 ? end : w * 32 + 32) - w * 32;
+      atomicOr(&pin[w], (hi - lo == 32 ? full : (1u << (hi - lo)) - 1u) << lo);
+    }
+  }
+  __syncwarp();
+  const bool good0 = pin[0] & 1u;
+  auto stops = [&](int p, uint32_t lim) {   // position p ends the segment (rle_segment_end's loop test)
+    return p >= length || ((pin[p >> 5] >> (p & 31)) & 1u) || !rle_extends(counts[p], lim);
+  };
+  // every position's segment end, as far as 32 counts ahead, by the lane that owns it
+  for (int a = lane; a < length; a += 32) {
+    const uint32_t lim = rle_segment_limit(counts, length, good0, a);
+    int b = a + 1;
+    while (b <= a + 32 && !stops(b, lim)) b++;
+    ends[a] = b <= a + 32 ? (uint32_t)b : 0u;
+  }
+  __syncwarp();
+  // hop through the reached starts: one shared-memory load per segment; a segment longer than 32 is
+  // followed by the whole warp, 32 positions per ballot
+  uint32_t segw = 0;   // lane w: the segment starts among positions [32w, 32w + 32)
+  for (int a = 0; a < length;) {
+    if ((int)lane == (a >> 5)) segw |= 1u << (a & 31);
+    int b = (int)ends[a];
+    if (b == 0) {
+      const uint32_t lim = rle_segment_limit(counts, length, good0, a);
+      for (int base = a + 33;; base += 32) {
+        const uint32_t m = __ballot_sync(full, stops(base + (int)lane, lim));
+        if (m) { b = base + __ffs(m) - 1; break; }
+      }
+    }
+    a = b;
+  }
+  if ((int)lane < nw) seg[lane] = segw;
+  __syncwarp();
+  for (int a = lane; a < length; a += 32) {
+    if (!((seg[a >> 5] >> (a & 31)) & 1u)) continue;
+    const int end = next_mark(seg, nw, a, length);
+    uint64_t sum = 0;
+    for (int k = a; k < end; k++) sum += counts[k];
+    uint32_t mean;
+    if (rle_flatten(sum, end - a, &mean))
+      for (int k = a; k < end; k++) counts[k] = mean;
+  }
+  __syncwarp();
 }
 
 __device__ uint64_t warp_dynamic_bits(const uint32_t* hist, CostStage& cs, uint32_t lane, DynChoice* choice = nullptr) {
-  // RLE-smoothed copies of both histograms (TryOptimizeHuffmanForRle deflate.c:525-567): two
-  // serial scans side by side, then four warp-wide code constructions
+  // RLE-smoothed copies of both histograms (TryOptimizeHuffmanForRle deflate.c:525-567), then four
+  // warp-wide code constructions
   for (int i = lane; i < 320; i += 32) cs.cnt2[i] = hist[i];
   __syncwarp();
-  if (lane < 2) optimize_for_rle(lane ? kNumD : kNumLL, cs.cnt2 + (lane ? 288 : 0), cs.good + (lane ? 288 : 0));
-  __syncwarp();
+  warp_optimize_for_rle(cs.cnt2, kNumLL, cs.pm, lane);
+  warp_optimize_for_rle(cs.cnt2 + 288, kNumD, cs.pm, lane);
   warp_length_limited(hist, kNumLL, cs.len[0], cs.pm, lane);
   warp_length_limited(hist + 288, kNumD, cs.len[0] + 288, cs.pm, lane);
   warp_length_limited(cs.cnt2, kNumLL, cs.len[1], cs.pm, lane);

@@ -10,6 +10,11 @@
 #else
 #define ZB_HD inline
 #endif
+#if defined(__CUDA_ARCH__)
+#define ZB_UNROLL _Pragma("unroll")
+#else
+#define ZB_UNROLL
+#endif
 
 namespace zb {
 
