@@ -163,6 +163,53 @@ void ZopfliB200FreeDevice(void* dev_ptr, void* cuda_stream); /* cudaFreeAsync on
 int ZopfliB200Crc32Device(const unsigned char* dev_in, size_t size, void* cuda_stream, uint32_t* crc);
 int ZopfliB200Adler32Device(const unsigned char* dev_in, size_t size, void* cuda_stream, uint32_t* adler);
 
+/* ---- input in pieces ----
+ * A compressor takes its input in pieces (chunks) and returns the bytes ZopfliCompress returns for all of them
+ * concatenated, in bounded memory, like zlib's deflate stream.  Master block i (deflate.c:908-931) depends only
+ * on its bytes, the 32 KiB before it and whether it is the last one, so the compressor runs the input as waves
+ * of whole master blocks (half as many as ZopfliCompress runs at once on the device, so that the two waves in
+ * flight fit the device memory of one call: about 72 on an 80 GB card by the driver's schedule; ZOPFLI_B200_BATCH and ZOPFLI_B200_CHUNKS shrink them) while more bytes arrive.
+ *  - Identical bytes: every Write output followed by the Finish output, concatenated, equals
+ *    ZopfliCompress(options, output_type, <all chunks concatenated>), for every chunking (zero-length writes
+ *    included) and all three formats.  A compressor finished at once gives ZopfliCompress of an empty input.
+ *  - Ownership: *out / *outsize follow ZopfliCompress's rule (bytes are appended under zopfli's capacity rule,
+ *    the caller frees).  Only complete bytes are returned; the compressor keeps the partly filled last byte.
+ *    The gzip / zlib header comes out with the first Write that returns bytes, or with Finish.
+ *  - Chunks: device < 0: chunks are host memory.  device >= 0: chunks are memory of that device, and each
+ *    Write is ordered after the work queued on cuda_stream (a stream of that device, NULL = legacy default
+ *    stream).  A chunk may be reused or freed as soon as Write returns; for device chunks Write waits for its
+ *    own device-to-device copy, not for the compression.  A full master block is compressed once a byte past
+ *    it has arrived, so a Write may return no bytes.
+ *  - Errors: Write and Finish return nonzero and leave every output untouched for a NULL c, out or outsize,
+ *    device memory given to a host compressor, host memory or another device's memory given to a device
+ *    compressor (n > 0), and any call after Finish.  New returns nonzero, *c untouched, for NULL options or
+ *    c, an unknown format, or a device that does not exist.
+ *  - Threads: one compressor is used by one thread at a time; different compressors may run at the same time
+ *    from any threads.  One compressor runs on one GPU: ZOPFLI_B200_GPUS does not apply.
+ *  - Reports: Finish updates ZopfliB200LastMasterBitOffsets to the whole stream's offsets (those ZopfliCompress
+ *    leaves for the same input).  With verbose, each wave prints its reports as ZopfliCompress does, waves
+ *    running one at a time, and Finish prints the size reports: a one-wave input prints what ZopfliCompress
+ *    prints.
+ *  - Memory: at most two waves are in flight and one fills; a Write that completes a third wave waits for the
+ *    oldest.  The staging a compressor holds (host memory, or device memory for device chunks) is at most
+ *    three slots of one wave plus its dictionary each: 3 x (wave bytes + 32 KiB + 16), whatever the total
+ *    length.  Output not yet returned is at most one byte between calls. */
+typedef struct ZopfliB200Compressor ZopfliB200Compressor;
+int ZopfliB200CompressorNew(const ZopfliOptions* options, ZopfliFormat output_type, int device, void* cuda_stream,
+                            ZopfliB200Compressor** c);
+/* Appends to (*out, *outsize), zopfli-style, whatever output bytes are complete.  May return none. */
+int ZopfliB200CompressorWrite(ZopfliB200Compressor* c, const unsigned char* chunk, size_t n, unsigned char** out,
+                              size_t* outsize);
+/* Compresses the rest and appends it together with the trailer. */
+int ZopfliB200CompressorFinish(ZopfliB200Compressor* c, unsigned char** out, size_t* outsize);
+/* Also valid before Finish: abandons the work (waits for the waves in flight, drops their output). */
+void ZopfliB200CompressorFree(ZopfliB200Compressor* c);
+/* The compressor's wave policy as a pure function (csrc/dist_layout.hpp next_wave; no GPU needed): with
+ * `received` bytes written, Finish called or not, `handed` bytes already in waves and waves of wave_blocks
+ * master blocks, returns 1 and the next wave [*a, *b) with its BFINAL flag, or 0 when no wave is ready. */
+int ZopfliB200CompressorWave(size_t received, int finished, size_t handed, size_t wave_blocks, size_t* a, size_t* b,
+                             int* final);
+
 /* ---- several GPUs, one stream (SURVEY 8(e)) ----
  * The master blocks of one input (the reference's independent unit, deflate.c:908-931) are sharded
  * over the GPUs of one box; NCCL scatters the byte ranges (+ 32 KiB dictionary) from rank 0's GPU and
@@ -193,8 +240,10 @@ void ZopfliB200DistPlacement(const uint64_t* len8, int world, unsigned phase0, u
 /* CRC-32 of the gzip trailer (gzip_container.c:27-81) and its combination across shards. */
 uint32_t ZopfliB200Crc32(const unsigned char* data, size_t size);
 uint32_t ZopfliB200Crc32Combine(uint32_t crc1, uint32_t crc2, uint64_t len2);
-/* Adler-32 of the zlib trailer (zlib_container.c:29-48), threaded with an exact combination. */
+/* Adler-32 of the zlib trailer (zlib_container.c:29-48), threaded with an exact combination, and the
+ * combination of consecutive slices (adler32 of A|B from those of A and B and |B|). */
 uint32_t ZopfliB200Adler32(const unsigned char* data, size_t size);
+uint32_t ZopfliB200Adler32Combine(uint32_t adler1, uint32_t adler2, uint64_t len2);
 /* The slice algebra of the device checksums (csrc/checksum.hpp) run on the host: the input cut into
  * slices of slice_bytes, each reduced on its own and combined.  kind 0: CRC-32, 1: Adler-32. */
 uint32_t ZopfliB200HostChecksumSliced(const unsigned char* data, size_t size, size_t slice_bytes, int kind);

@@ -52,11 +52,12 @@ EXPORTS = ["ZopfliInitOptions", "ZopfliCompress", "ZopfliDeflate", "ZopfliDeflat
            "ZopfliB200MatchTable", "ZopfliB200DynamicBlockBits", "ZopfliB200DeviceAutoTypeBits", "ZopfliB200HostBlockSplitLZ77",
            "ZopfliB200HostBatchedSplit", "ZopfliB200HostBlockSize", "ZopfliB200HostEmitBlock", "ZopfliB200DeviceEmitBlocks", "ZopfliB200HostEmitBlocks", "ZopfliB200HostLengthLimited", "ZopfliB200HostOptimizeRle",
            "ZopfliB200HostOptimizeRleBatch", "ZopfliB200HostTreeHeaderBits", "ZopfliB200HostProbeParts", "ZopfliB200DeviceProbeParts",
-           "ZopfliB200DeflateSpan", "ZopfliB200AppendSpan", "ZopfliB200LastMasterBitOffsets", "ZopfliB200Crc32", "ZopfliB200Crc32Combine", "ZopfliB200Adler32", "ZopfliB200CompressDevice",
+           "ZopfliB200DeflateSpan", "ZopfliB200AppendSpan", "ZopfliB200LastMasterBitOffsets", "ZopfliB200Crc32", "ZopfliB200Crc32Combine", "ZopfliB200Adler32", "ZopfliB200Adler32Combine", "ZopfliB200CompressDevice",
            "ZopfliB200DistUniqueId", "ZopfliB200DistInit", "ZopfliB200DistCompress", "ZopfliB200DistFinalize", "ZopfliB200DistShard", "ZopfliB200DistPlacement",
            "ZopfliB200GetStats", "ZopfliB200ResetStats", "ZopfliB200SetStream", "ZopfliB200Device",
            "ZopfliB200Version", "ZopfliB200CompressDeviceToDevice", "ZopfliB200FreeDevice", "ZopfliB200Crc32Device",
-           "ZopfliB200Adler32Device", "ZopfliB200HostChecksumSliced"]
+           "ZopfliB200Adler32Device", "ZopfliB200HostChecksumSliced", "ZopfliB200CompressorNew", "ZopfliB200CompressorWrite",
+           "ZopfliB200CompressorFinish", "ZopfliB200CompressorFree", "ZopfliB200CompressorWave"]
 
 
 def _pad(data):
@@ -197,8 +198,20 @@ class Library:
         L.ZopfliB200Crc32Combine.restype = C.c_uint32
         L.ZopfliB200Adler32.argtypes = [vp, sz]
         L.ZopfliB200Adler32.restype = C.c_uint32
+        L.ZopfliB200Adler32Combine.argtypes = [C.c_uint32, C.c_uint32, C.c_uint64]
+        L.ZopfliB200Adler32Combine.restype = C.c_uint32
         L.ZopfliB200HostChecksumSliced.argtypes = [vp, sz, sz, C.c_int]
         L.ZopfliB200HostChecksumSliced.restype = C.c_uint32
+        L.ZopfliB200CompressorNew.argtypes = [C.POINTER(ZopfliOptions), C.c_int, C.c_int, vp, C.POINTER(vp)]
+        L.ZopfliB200CompressorNew.restype = C.c_int
+        L.ZopfliB200CompressorWrite.argtypes = [vp, vp, sz, C.POINTER(vp), C.POINTER(sz)]
+        L.ZopfliB200CompressorWrite.restype = C.c_int
+        L.ZopfliB200CompressorFinish.argtypes = [vp, C.POINTER(vp), C.POINTER(sz)]
+        L.ZopfliB200CompressorFinish.restype = C.c_int
+        L.ZopfliB200CompressorFree.argtypes = [vp]
+        L.ZopfliB200CompressorFree.restype = None
+        L.ZopfliB200CompressorWave.argtypes = [sz, C.c_int, sz, sz, C.POINTER(sz), C.POINTER(sz), C.POINTER(C.c_int)]
+        L.ZopfliB200CompressorWave.restype = C.c_int
         # device-resident calls and the device emission seam (csrc/device_api.cpp); a host-only test build of the
         # ABI does not export them
         for name, args, res in (("ZopfliB200CompressDeviceToDevice",
@@ -467,6 +480,9 @@ class Library:
     def crc32_combine(self, crc1, crc2, len2) -> int:
         return int(self.lib.ZopfliB200Crc32Combine(crc1, crc2, len2))
 
+    def adler32_combine(self, adler1, adler2, len2) -> int:
+        return int(self.lib.ZopfliB200Adler32Combine(adler1, adler2, len2))
+
     def host_checksum_sliced(self, data: bytes, slice_bytes: int, kind: int) -> int:
         """the device checksums' slice algebra on the host; kind 0 CRC-32, 1 Adler-32"""
         a = _pad(data)
@@ -505,6 +521,23 @@ class Library:
     def adler32_device(self, t, stream=None) -> int:
         """zlib.adler32 of the raw bytes of a contiguous CUDA tensor, computed on its device"""
         return self._device_checksum(self.lib.ZopfliB200Adler32Device, t, stream)
+
+    # ---- input in pieces (ZopfliB200Compressor) ----
+    def compressobj(self, fmt=ZOPFLI_FORMAT_GZIP, device=None, stream=None, **kw) -> "Compressor":
+        """A compressor shaped like zlib.compressobj: compress(chunk) -> bytes, flush() -> bytes.  All outputs
+        concatenated equal compress(<all chunks>, fmt, **kw).  device=None: chunks are bytes-like objects;
+        device=<index or torch.device>: chunks are contiguous CUDA tensors of that device, each copied after
+        the work queued on `stream`, or, without stream=, on the tensor's current stream (a private stream of the
+        compressor waits for it, so the caller's streams gain no dependency)."""
+        return Compressor(self, fmt, device, stream, **kw)
+
+    def compressor_wave(self, received, finished, handed, wave_blocks):
+        """the compressor's next wave (a, b, final), or None (ZopfliB200CompressorWave)"""
+        a, b, f = C.c_size_t(0), C.c_size_t(0), C.c_int(0)
+        if not self.lib.ZopfliB200CompressorWave(received, 1 if finished else 0, handed, wave_blocks, C.byref(a), C.byref(b),
+                                                 C.byref(f)):
+            return None
+        return a.value, b.value, bool(f.value)
 
     def splice_spans(self, spans, prefix=b"", bp0=0) -> tuple[bytes, int]:
         """appends spans behind `prefix`, whose last byte has bp0 bits in use -> (bytes, final bp)"""
@@ -582,6 +615,73 @@ class Library:
         return self.lib.ZopfliB200Version().decode()
 
 
+class Compressor:
+    """ZopfliB200Compressor: input in pieces, ZopfliCompress's bytes out (include/zopfli_b200.h, "input in
+    pieces").  Use it as a context manager, or close() it; closing an unfinished compressor abandons it."""
+
+    def __init__(self, lib, fmt=ZOPFLI_FORMAT_GZIP, device=None, stream=None, **kw):
+        self._c = None
+        self._lib, self._stream = lib, None
+        dev = -1
+        if device is not None:
+            import torch
+            dev = torch.device("cuda", device) if isinstance(device, int) else torch.device(device)
+            dev = dev.index if dev.index is not None else torch.cuda.current_device()
+            if stream is None:
+                # a stream of the compressor's own: each chunk's copy waits for the chunk's current stream through
+                # it (compress), so no stream of the caller's gains a dependency
+                self._stream = torch.cuda.Stream(device=dev)
+            elif hasattr(stream, "cuda_stream"):
+                self._stream = stream
+            else:
+                self._stream = torch.cuda.ExternalStream(int(stream), device=torch.device("cuda", dev))
+        self._dev, self._own_stream = dev, stream is not None
+        handle = C.c_void_p(None)
+        o = lib.options(**kw)
+        if lib.lib.ZopfliB200CompressorNew(C.byref(o), fmt, dev, self._stream.cuda_stream if dev >= 0 else None,
+                                           C.byref(handle)) != 0:
+            raise ValueError("ZopfliB200CompressorNew: unknown format, or no such device")
+        self._c = handle
+
+    def _call(self, fn, *args):
+        if self._c is None:
+            raise ValueError("compressor is closed")
+        out, n = C.c_void_p(None), C.c_size_t(0)
+        if fn(self._c, *args, C.byref(out), C.byref(n)) != 0:
+            raise ValueError("compressor refused the call: it is finished, or the chunk is the wrong kind of memory")
+        return self._lib._take(out, n)
+
+    def compress(self, chunk) -> bytes:
+        """the output bytes that are complete after this chunk (possibly none)"""
+        if self._dev >= 0:
+            import torch
+            if not isinstance(chunk, torch.Tensor):
+                raise ValueError("a device compressor takes CUDA tensors")
+            ptr, nbytes = _device_bytes(chunk)
+            if not self._own_stream:  # ordered after the chunk's current stream, as compress_device is
+                self._stream.wait_stream(torch.cuda.current_stream(chunk.device))
+            return self._call(self._lib.lib.ZopfliB200CompressorWrite, C.c_void_p(ptr), nbytes)
+        a = np.frombuffer(memoryview(chunk).cast("B"), np.uint8)
+        return self._call(self._lib.lib.ZopfliB200CompressorWrite, a.ctypes.data if len(a) else None, len(a))
+
+    def flush(self) -> bytes:
+        """the rest of the stream with the trailer; the compressor takes no more input"""
+        return self._call(self._lib.lib.ZopfliB200CompressorFinish)
+
+    def close(self):
+        if self._c is not None:
+            self._lib.lib.ZopfliB200CompressorFree(self._c)
+            self._c = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    __del__ = close
+
+
 _default = None
 
 
@@ -595,3 +695,8 @@ def library() -> Library:
 def compress(data: bytes, fmt: int = ZOPFLI_FORMAT_GZIP, **options) -> bytes:
     """ZopfliCompress with default ZopfliOptions unless overridden (numiterations=, ...)."""
     return library().compress(data, fmt, **options)
+
+
+def compressobj(fmt: int = ZOPFLI_FORMAT_GZIP, device=None, stream=None, **options) -> Compressor:
+    """a compressor fed in pieces (Library.compressobj), like zlib.compressobj"""
+    return library().compressobj(fmt, device, stream, **options)

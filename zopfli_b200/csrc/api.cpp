@@ -7,6 +7,9 @@
 #include <string.h>
 
 #include <algorithm>
+#include <atomic>
+#include <deque>
+#include <memory>
 #include <mutex>
 #include <thread>
 #include <vector>
@@ -99,6 +102,59 @@ void seam_plan_out(const BlockPlan& b, Piece& p, unsigned char* len320, uint64_t
   memcpy(val6, v, sizeof(v));
   p.nbits = p.type == 1 ? b.fixed_bits : b.dyn_bits;
   p.tree_bits = b.tree_bits;
+}
+
+void deflate_span_records(Engine& eng, const ZopfliOptions* opt, size_t base, size_t start, size_t end, bool final,
+                          const std::function<void(size_t, size_t, unsigned char*)>& read, SpanRecords& out) {
+  std::vector<Piece>& pieces = out.pieces;
+  pieces.clear();
+  out.recs.clear();
+  deflate_units(eng, opt, 2, final, master_blocks(start, end), base, pieces);
+  // Records: maximal runs of compressed pieces, each emitted on the device from bit offset 0 of a
+  // byte-aligned slot of one download buffer, and stored pieces as raw bytes.
+  std::vector<std::pair<size_t, uint64_t>> runs;    // (record, first bit in the download buffer)
+  std::vector<std::pair<size_t, size_t>> stored;    // (record, piece)
+  std::vector<Engine::EmitPiece> ep_all;
+  uint64_t pos = 0;
+  size_t nstored = 0;
+  for (size_t i = 0; i < pieces.size();) {
+    SpanPiece r;
+    if (pieces[i].type == 0) {
+      r.stored = true;
+      r.final = pieces[i].final;
+      r.instart = nstored;
+      nstored += pieces[i].inend - pieces[i].instart;
+      r.inend = nstored;
+      stored.push_back({out.recs.size(), i});
+      out.recs.push_back(std::move(r));
+      i++;
+      continue;
+    }
+    size_t j = i;
+    while (j < pieces.size() && pieces[j].type != 0) j++;
+    std::vector<Piece> run(pieces.begin() + i, pieces.begin() + j);
+    std::vector<Engine::EmitPiece> ep;
+    const uint64_t e = layout_pieces(run, base, pos, ep, nullptr);
+    r.final = pieces[j - 1].final;
+    r.bits.nbits = e - pos;
+    runs.push_back({out.recs.size(), pos});
+    out.recs.push_back(std::move(r));
+    ep_all.insert(ep_all.end(), ep.begin(), ep.end());
+    pos = (e + 63) & ~(uint64_t)63;  // the next run starts on a fresh word: no shared bytes between records
+    i = j;
+  }
+  std::vector<unsigned char> bits((size_t)(pos / 8) + 8, 0);
+  if (pos) eng.emit(ep_all, pos, bits.data());
+  for (const auto& r : runs) {
+    BitString& b = out.recs[r.first].bits;
+    const unsigned char* s = bits.data() + r.second / 8;
+    b.bytes.assign(s, s + (size_t)((b.nbits + 7) / 8));
+  }
+  out.stored.resize(nstored);
+  for (const auto& s : stored) {
+    const Piece& p = pieces[s.second];
+    if (p.inend > p.instart) read(p.instart, p.inend - p.instart, out.stored.data() + out.recs[s.first].instart);
+  }
 }
 
 }  // namespace zb
@@ -253,7 +309,225 @@ void make_store(const unsigned short* ll, const unsigned short* dd, size_t n, Lz
   st.finalize();
 }
 
+// A compressor's waves in host memory: one buffer per slot, reserved up to the bytes of one staged wave
+struct HostStaging : WaveStaging {
+  std::vector<unsigned char> slot[kSlots];
+  int device() const override { return -1; }
+  bool accepts(const void* p, size_t n) const override {
+    return n == 0 || (p && !(g_pointer_device && g_pointer_device(p) >= 0));
+  }
+  void put(int s, size_t off, const unsigned char* chunk, size_t n) override {
+    std::vector<unsigned char>& b = slot[s];
+    if (b.capacity() < off + n) b.reserve(std::max(off + n, std::min(2 * b.capacity(), slot_bytes)));
+    b.resize(off);
+    b.insert(b.end(), chunk, chunk + n);
+  }
+  void carry(int from, size_t off, int to, size_t n) override { put(to, 0, slot[from].data() + off, n); }
+  const unsigned char* at(int s, size_t off) {
+    static const unsigned char none[16] = {0};
+    return slot[s].empty() ? none : slot[s].data() + off;
+  }
+  void stage(Engine& eng, int s, size_t len) override { eng.set_input_host(at(s, 0), len); }
+  uint32_t checksum(Engine&, int s, size_t off, size_t n, int kind) override {
+    return kind == kCkCrc32 ? crc32_parallel(at(s, off), n) : adler32(at(s, off), n);
+  }
+  void read(Engine&, int s, size_t off, size_t n, unsigned char* dst) override { memcpy(dst, at(s, off), n); }
+};
+
 }  // namespace
+
+namespace zb {
+WaveStaging* (*g_device_staging)(int, void*) = nullptr;
+int (*g_pointer_device)(const void*) = nullptr;
+}  // namespace zb
+
+// ---- input in pieces (include/zopfli_b200.h) ----
+// Bytes are put into the filling slot of the staging; once a byte past a whole wave has arrived (next_wave),
+// the wave runs on a worker thread of its own, which leases an engine context for just that wave and turns it
+// into span records plus the checksum of its bytes.  The next wave's slot takes over the last 32 KiB as its
+// dictionary.  Waves are spliced onto the stream in order, at its bit phase, by the calling thread; only the
+// complete bytes go back to the caller.
+struct ZopfliB200Compressor {
+  struct Run {
+    Wave w;
+    size_t base;        // stream position of the slot's byte 0
+    int slot;
+    SpanRecords sr;
+    uint32_t sum = 0;   // checksum of the wave's bytes [w.a, w.b)
+    std::atomic<bool> done{false};
+    std::thread worker;
+  };
+
+  ZopfliOptions opt;
+  ZopfliFormat fmt;
+  int kind;
+  std::unique_ptr<WaveStaging> staging;
+  size_t wave_blocks = 0;            // master blocks per wave, set when the first byte arrives
+  size_t received = 0, handed = 0;   // bytes written; bytes that belong to waves
+  bool finished = false;
+  int fill = -1;                     // slot taking the next bytes (-1: none yet)
+  size_t fill_base = 0;              // stream position of its byte 0
+  std::vector<int> free_slots;
+  std::deque<std::unique_ptr<Run>> inflight;
+  // the stream not yet returned: at most the partly filled last byte between calls (zopfli-style buffer)
+  unsigned char* pend = nullptr;
+  size_t pendsize = 0;
+  unsigned char bp = 0;
+  bool header_done = false;
+  uint64_t deflate_bits = 0;         // bits of the deflate stream spliced so far
+  size_t produced = 0;               // bytes returned so far
+  uint32_t sum;                      // checksum of the bytes of the spliced waves
+  std::vector<uint64_t> layout;      // bit offset of every master block spliced so far
+  double busy_ms = 0;                // time spent in Write and Finish
+
+  ZopfliB200Compressor(const ZopfliOptions* o, ZopfliFormat f, WaveStaging* st)
+      : opt(*o), fmt(f), kind(f == ZOPFLI_FORMAT_GZIP ? kCkCrc32 : (f == ZOPFLI_FORMAT_ZLIB ? kCkAdler32 : kCkNone)),
+        staging(st), sum(kind == kCkAdler32 ? 1u : 0u) {
+    for (int s = WaveStaging::kSlots - 1; s >= 0; s--) free_slots.push_back(s);
+  }
+  ~ZopfliB200Compressor() {  // abandons unfinished work: waits for the waves in flight, drops their output
+    for (auto& r : inflight) r->worker.join();
+    free(pend);
+  }
+
+  // With verbose reports a wave starts once the one before it is spliced, so reports do not interleave.
+  size_t max_inflight() const { return (opt.verbose || opt.verbose_more) ? 1 : 2; }
+
+  void set_wave_blocks() {
+    if (wave_blocks) return;
+    Engine::Lease eng(staging->device());
+    wave_blocks = wave_master_blocks(eng->device_memory_total() / 2);  // two waves in flight: one call's budget
+    staging->slot_bytes = wave_blocks * kMasterBlock + kWindow + 16;
+  }
+
+  // the caller's bytes up to stream position `upto` into the filling slot; chunk starts at position `at`
+  void fill_to(size_t upto, const unsigned char* chunk, size_t at) {
+    if (upto == received) return;
+    if (fill < 0) take_slot(0);
+    staging->put(fill, received - fill_base, chunk + (received - at), upto - received);
+    received = upto;
+  }
+
+  void take_slot(size_t base) {
+    fill = free_slots.back();
+    free_slots.pop_back();
+    fill_base = base;
+  }
+
+  // runs on the wave's worker thread
+  void compress(Run& r) {
+    Engine::Lease eng(staging->device());
+    staging->stage(*eng, r.slot, r.w.b - r.base);
+    const size_t off = r.w.a - r.base, n = r.w.b - r.w.a;
+    std::thread ck;
+    if (kind != kCkNone) {
+      if (staging->device() < 0) ck = std::thread([&] { r.sum = staging->checksum(*eng, r.slot, off, n, kind); });  // overlaps the GPU work
+      else r.sum = staging->checksum(*eng, r.slot, off, n, kind);
+    }
+    deflate_span_records(*eng, &opt, r.base, r.w.a, r.w.b, r.w.final,
+                         [&](size_t pos, size_t len, unsigned char* dst) { staging->read(*eng, r.slot, pos - r.base, len, dst); },
+                         r.sr);
+    if (ck.joinable()) ck.join();
+    r.done = true;
+  }
+
+  // starts wave w on the filling slot; a wave that is not the last hands its last 32 KiB to a fresh slot
+  void launch(const Wave& w) {
+    while (inflight.size() >= max_inflight()) retire_oldest();
+    if (fill < 0) take_slot(0);  // an empty stream
+    std::unique_ptr<Run> r(new Run);
+    r->w = w;
+    r->base = fill_base;
+    r->slot = fill;
+    Run* p = r.get();
+    p->worker = std::thread([this, p] { compress(*p); });
+    inflight.push_back(std::move(r));
+    handed = w.b;
+    fill = -1;
+    if (w.final) return;
+    const size_t base = wave_base(w.b);
+    take_slot(base);
+    staging->carry(p->slot, base - p->base, fill, w.b - base);
+  }
+
+  // the oldest wave in flight, once done, spliced onto the stream (with the block reports of verbose)
+  void retire_oldest() {
+    std::unique_ptr<Run> r = std::move(inflight.front());
+    inflight.pop_front();
+    r->worker.join();
+    if (!header_done) {
+      unsigned char hdr[10];
+      append_bytes(hdr, container_header(fmt, hdr), &pend, &pendsize);
+      header_done = true;
+    }
+    const unsigned phase = pendsize ? (bp & 7u) : 0u;
+    std::vector<Engine::EmitPiece> ep;
+    std::vector<uint64_t> ub;
+    const uint64_t end = place_pieces(r->sr.pieces, r->base, phase, ep, &ub, opt.verbose != 0);
+    for (size_t i = 0; i + 1 < ub.size(); i++) layout.push_back(deflate_bits + ub[i]);
+    deflate_bits += end - phase;
+    splice_pieces(r->sr.recs, r->sr.stored.data(), &bp, &pend, &pendsize);
+    const uint64_t n = r->w.b - r->w.a;
+    if (kind == kCkCrc32) sum = crc32_combine(sum, r->sum, n);
+    else if (kind == kCkAdler32) sum = adler32_combine(sum, r->sum, n);
+    free_slots.push_back(r->slot);
+  }
+
+  // appends the complete bytes (all of them with `all`) to the caller's buffer
+  // appends the complete bytes (all of them with `all`) to the caller's buffer.  What stays behind is at most
+  // the partly filled last byte, in a fresh one-byte buffer: zopfli's capacity rule derives a buffer's
+  // capacity from its size, so a larger buffer must not be kept under a smaller size.
+  void hand_out(unsigned char** out, size_t* outsize, bool all) {
+    const size_t keep = (!all && bp != 0 && pendsize > 0) ? 1 : 0;
+    const unsigned char last = keep ? pend[pendsize - 1] : 0;
+    append_bytes(pend, pendsize - keep, out, outsize);
+    produced += pendsize - keep;
+    free(pend);
+    pend = nullptr;
+    pendsize = 0;
+    if (keep) append_bytes(&last, 1, &pend, &pendsize);
+  }
+
+  int write(const unsigned char* chunk, size_t n, unsigned char** out, size_t* outsize) {
+    if (!out || !outsize || finished || !staging->accepts(chunk, n)) return 1;
+    const double t0 = now_ms();
+    if (n) {
+      set_wave_blocks();
+      const size_t at = received, total = received + n;
+      Wave w;
+      while (next_wave(total, false, handed, wave_blocks, &w)) {
+        fill_to(w.b, chunk, at);
+        launch(w);
+      }
+      fill_to(total, chunk, at);
+    }
+    while (!inflight.empty() && inflight.front()->done) retire_oldest();
+    hand_out(out, outsize, false);
+    busy_ms += now_ms() - t0;
+    return 0;
+  }
+
+  int finish(unsigned char** out, size_t* outsize) {
+    if (!out || !outsize || finished) return 1;
+    const double t0 = now_ms();
+    finished = true;
+    Wave w;
+    next_wave(received, true, handed, wave_blocks, &w);
+    launch(w);
+    while (!inflight.empty()) retire_oldest();
+    unsigned char tr[8];
+    append_bytes(tr, container_trailer(kind, sum, received, tr), &pend, &pendsize);
+    hand_out(out, outsize, true);
+    if (opt.verbose) {  // the reports ZopfliCompress prints after the deflate body and after the container
+      report_size(ZOPFLI_FORMAT_DEFLATE, received, (size_t)((deflate_bits + 7) / 8));
+      if (fmt != ZOPFLI_FORMAT_DEFLATE) report_size(fmt, received, produced);
+    }
+    layout.push_back(deflate_bits);
+    busy_ms += now_ms() - t0;
+    api_call_done(layout, now_ms() - busy_ms);
+    return 0;
+  }
+};
 
 extern "C" {
 
@@ -323,48 +597,27 @@ int ZopfliB200DeflateSpan(const ZopfliOptions* options, const unsigned char* in,
                           unsigned char** span, size_t* spansize) {
   if (end > insize || start > end) return 1;
   if (start == end && insize > 0) return 0;  // an empty span of an empty input is one empty master block
-  std::vector<Piece> pieces;
   size_t base = 0;
   Engine::Lease eng;
   if (dev_in) {
     eng->set_input_device(dev_in, insize);
   } else {
-    base = start > (size_t)kWindow ? start - kWindow : 0;
-    base &= ~(size_t)15;
+    base = wave_base(start);
     eng->set_input_host(in + base, end - base);
   }
-  deflate_units(*eng, options, 2, final != 0, master_blocks(start, end), base, pieces);
-  // Records: maximal runs of compressed pieces, each emitted on the device from bit offset 0 of a
-  // byte-aligned slot of one download buffer, and stored pieces as raw bytes.
-  struct Rec { bool stored; bool final; size_t first, count; uint64_t bit0, nbits; };
-  std::vector<Rec> recs;
-  std::vector<Engine::EmitPiece> ep_all;
-  uint64_t pos = 0;
-  for (size_t i = 0; i < pieces.size();) {
-    if (pieces[i].type == 0) { recs.push_back({true, pieces[i].final, i, 1, 0, 0}); i++; continue; }
-    size_t j = i;
-    while (j < pieces.size() && pieces[j].type != 0) j++;
-    std::vector<Piece> run(pieces.begin() + i, pieces.begin() + j);
-    std::vector<Engine::EmitPiece> ep;
-    const uint64_t end = layout_pieces(run, base, pos, ep, nullptr);
-    recs.push_back({false, pieces[j - 1].final, i, j - i, pos, end - pos});
-    ep_all.insert(ep_all.end(), ep.begin(), ep.end());
-    pos = (end + 63) & ~(uint64_t)63;  // the next run starts on a fresh word: no shared bytes between records
-    i = j;
-  }
-  std::vector<unsigned char> bits((size_t)(pos / 8) + 8, 0);
-  if (pos) eng->emit(ep_all, pos, bits.data());
+  SpanRecords sr;
+  deflate_span_records(*eng, options, base, start, end, final != 0,
+                       [&](size_t pos, size_t n, unsigned char* dst) { memcpy(dst, in + pos, n); }, sr);
   size_t total = 0;
-  for (const Rec& r : recs) total += 10 + (r.stored ? pieces[r.first].inend - pieces[r.first].instart : (size_t)((r.nbits + 7) / 8));
+  for (const SpanPiece& r : sr.recs) total += 10 + (r.stored ? r.inend - r.instart : r.bits.bytes.size());
   unsigned char* d = append_reserve(total, span, spansize);
-  for (const Rec& r : recs) {
+  for (const SpanPiece& r : sr.recs) {
     d[0] = r.stored ? 1 : 0;
     d[1] = r.final ? 1 : 0;
-    const uint64_t v = r.stored ? (uint64_t)(pieces[r.first].inend - pieces[r.first].instart) : r.nbits;
+    const uint64_t v = r.stored ? (uint64_t)(r.inend - r.instart) : r.bits.nbits;
     memcpy(d + 2, &v, 8);
-    const size_t nb = r.stored ? (size_t)v : (size_t)((v + 7) / 8);
-    if (r.stored) memcpy(d + 10, in + pieces[r.first].instart, nb);
-    else memcpy(d + 10, bits.data() + r.bit0 / 8, nb);
+    const size_t nb = r.stored ? (size_t)v : r.bits.bytes.size();
+    if (nb) memcpy(d + 10, r.stored ? sr.stored.data() + r.instart : r.bits.bytes.data(), nb);
     d += 10 + nb;
   }
   return 0;
@@ -372,6 +625,7 @@ int ZopfliB200DeflateSpan(const ZopfliOptions* options, const unsigned char* in,
 
 uint32_t ZopfliB200Crc32(const unsigned char* data, size_t size) { return crc32_parallel(data, size); }
 uint32_t ZopfliB200Crc32Combine(uint32_t crc1, uint32_t crc2, uint64_t len2) { return crc32_combine(crc1, crc2, len2); }
+uint32_t ZopfliB200Adler32Combine(uint32_t adler1, uint32_t adler2, uint64_t len2) { return adler32_combine(adler1, adler2, len2); }
 uint32_t ZopfliB200Adler32(const unsigned char* data, size_t size) { return adler32(data, size); }
 uint32_t ZopfliB200HostChecksumSliced(const unsigned char* data, size_t size, size_t slice_bytes, int kind) {
   return checksum_sliced(data, size, slice_bytes, kind);
@@ -414,6 +668,38 @@ int ZopfliB200AppendSpan(const unsigned char* span, size_t spansize, unsigned ch
   }
   splice_pieces(pieces, rawbytes.data(), bp, out, outsize);
   return 0;
+}
+
+int ZopfliB200CompressorNew(const ZopfliOptions* options, ZopfliFormat output_type, int device, void* cuda_stream,
+                            ZopfliB200Compressor** c) {
+  if (!options || !c) return 1;
+  if (output_type != ZOPFLI_FORMAT_GZIP && output_type != ZOPFLI_FORMAT_ZLIB && output_type != ZOPFLI_FORMAT_DEFLATE) return 1;
+  WaveStaging* st = nullptr;
+  if (device < 0) st = new HostStaging;
+  else if (!g_device_staging || !(st = g_device_staging(device, cuda_stream))) return 1;
+  *c = new ZopfliB200Compressor(options, output_type, st);
+  return 0;
+}
+
+int ZopfliB200CompressorWrite(ZopfliB200Compressor* c, const unsigned char* chunk, size_t n, unsigned char** out,
+                              size_t* outsize) {
+  return c ? c->write(chunk, n, out, outsize) : 1;
+}
+
+int ZopfliB200CompressorFinish(ZopfliB200Compressor* c, unsigned char** out, size_t* outsize) {
+  return c ? c->finish(out, outsize) : 1;
+}
+
+void ZopfliB200CompressorFree(ZopfliB200Compressor* c) { delete c; }
+
+int ZopfliB200CompressorWave(size_t received, int finished, size_t handed, size_t wave_blocks, size_t* a, size_t* b,
+                             int* final) {
+  Wave w;
+  if (!next_wave(received, finished != 0, handed, wave_blocks, &w)) return 0;
+  *a = w.a;
+  *b = w.b;
+  *final = w.final ? 1 : 0;
+  return 1;
 }
 
 size_t ZopfliB200LastMasterBitOffsets(uint64_t* offsets, size_t cap) {

@@ -4,6 +4,7 @@
 #include <stddef.h>
 #include <stdint.h>
 
+#include <functional>
 #include <vector>
 
 #include "../../include/zopfli.h"
@@ -12,6 +13,40 @@ namespace zb {
 
 struct BlockPlan;
 struct Piece;
+struct SpanRecords;
+class Engine;
+
+// ZopfliB200DeflateSpan's body: master blocks [start, end) of the input, whose bytes from position `base` on
+// the engine already holds, as span records.  read(pos, n, dst) copies input bytes [pos, pos + n) to the host:
+// the payloads of stored blocks.
+void deflate_span_records(Engine& eng, const ZopfliOptions* opt, size_t base, size_t start, size_t end, bool final,
+                          const std::function<void(size_t, size_t, unsigned char*)>& read, SpanRecords& out);
+
+// Where a compressor (ZopfliB200Compressor) keeps the bytes of its waves: host memory here, device memory in
+// device_api.cpp.  Slot s holds stream bytes from the slot's base on; it grows as bytes are put into it.
+struct WaveStaging {
+  static constexpr int kSlots = 3;  // two waves in flight and one filling
+  size_t slot_bytes = 0;            // the most a slot holds: one wave and its dictionary (set by the compressor)
+  virtual ~WaveStaging() {}
+  virtual int device() const = 0;  // -1: host memory
+  // whether a chunk of n bytes at p is memory of the kind this staging takes
+  virtual bool accepts(const void* p, size_t n) const = 0;
+  // slot s, offset off <- chunk[0, n) (the caller may reuse the chunk when put returns)
+  virtual void put(int s, size_t off, const unsigned char* chunk, size_t n) = 0;
+  // slot to, offset 0 <- slot from, bytes [off, off + n): the dictionary a wave takes over from the one before
+  virtual void carry(int from, size_t off, int to, size_t n) = 0;
+  // on a wave's worker, holding eng: slot s's bytes [0, len) become the engine's input
+  virtual void stage(Engine& eng, int s, size_t len) = 0;
+  // CRC-32 / Adler-32 (ChecksumKind) of slot s's bytes [off, off + n), with the engine set up by stage()
+  virtual uint32_t checksum(Engine& eng, int s, size_t off, size_t n, int kind) = 0;
+  // slot s's bytes [off, off + n) to dst
+  virtual void read(Engine& eng, int s, size_t off, size_t n, unsigned char* dst) = 0;
+};
+// The device side of ZopfliB200CompressorNew, registered by device_api.cpp (null in a host-only build): a
+// staging on device dev, ordered after cuda_stream, or null when dev is not a usable device.
+extern WaveStaging* (*g_device_staging)(int dev, void* cuda_stream);
+// device that owns p, else -1 (always -1 in a host-only build)
+extern int (*g_pointer_device)(const void* p);
 
 // a compression call that started at t0 (now_ms) is done: `layout` becomes what
 // ZopfliB200LastMasterBitOffsets returns, and the call's time is added to ZopfliB200Stats::ms_total

@@ -64,6 +64,15 @@ inline uint32_t crc32_combine(uint32_t crc1, uint32_t crc2, uint64_t len2) {
   return crc_shift(crc1, len2, t) ^ crc2;
 }
 
+// Adler-32 of A|B from adler32(A), adler32(B) and |B| (the zlib adler32_combine construction).  With s1 = 1 + sum
+// of bytes and s2 = sum of the s1 after each byte: s1(A|B) = s1(A) + s1(B) - 1, s2(A|B) = s2(A) + s2(B) + |B| (s1(A) - 1).
+inline uint32_t adler32_combine(uint32_t adler1, uint32_t adler2, uint64_t len2) {
+  const uint64_t a1 = adler1 & 0xffff, b1 = adler1 >> 16, a2 = adler2 & 0xffff, b2 = adler2 >> 16;
+  const uint64_t s1 = (a1 + a2 + kAdlerMod - 1) % kAdlerMod;
+  const uint64_t s2 = (b1 + b2 + (len2 % kAdlerMod) * ((a1 + kAdlerMod - 1) % kAdlerMod)) % kAdlerMod;
+  return (uint32_t)((s2 << 16) | s1);
+}
+
 // s1 = sum of bytes, s2 = sum of (n - i) * d_i over p[0, n), both mod 65521.  5552 bytes is the largest run
 // whose 32-bit running sums cannot overflow (the zlib bound the reference also relies on with 5550).
 struct AdlerPart { uint64_t s1, s2, len; };

@@ -1,8 +1,9 @@
 // C-ABI calls of libzopfli.so.1 whose input and result live in device memory (include/zopfli_b200.h,
 // "input and output in device memory"): the deflate pieces are the ones ZopfliCompress produces, the stream
 // is emitted behind the container header in a device allocation, and the checksum is computed on the device.
-// Also the device half of the block-emission seam (ZopfliB200DeviceEmitBlocks), which needs engine calls
-// the host-only test build of api.cpp does not have.
+// Also the device half of the block-emission seam (ZopfliB200DeviceEmitBlocks) and the device staging of
+// ZopfliB200Compressor, which need engine calls the host-only test build of api.cpp does not have.
+#include <algorithm>
 #include <vector>
 
 #include "../../include/zopfli_b200.h"
@@ -55,6 +56,69 @@ int device_checksum(const unsigned char* dev_in, size_t size, void* stream, int 
   *out = eng->checksum_device(dev_in, size, stream, kind);
   return 0;
 }
+
+// A compressor's waves in device memory (chunks of one device): one stream-ordered allocation per slot, grown
+// as bytes arrive up to one wave and its dictionary.  Each chunk is copied device to device after the work
+// queued on the caller's stream; a wave's engine adopts its slot as input (no host copy), and only the bytes of
+// stored blocks come back to the host.
+struct DeviceWaveStaging : WaveStaging {
+  DeviceStaging ds;
+  void* user_stream;
+  unsigned char* slot[kSlots] = {};
+  size_t cap[kSlots] = {}, len[kSlots] = {};
+  static constexpr size_t kPad = 64;  // the kernels read up to 16 bytes past the input; zeroed as set_input_host does
+
+  DeviceWaveStaging(int dev, void* stream) : ds(dev), user_stream(stream) {}
+  ~DeviceWaveStaging() override {
+    for (int s = 0; s < kSlots; s++) ds.release(slot[s]);
+  }
+  int device() const override { return ds.device(); }
+  bool accepts(const void* p, size_t n) const override { return n == 0 || Engine::pointer_device(p) == ds.device(); }
+  void grow(int s, size_t need) {  // keeps the slot's len[s] bytes
+    if (need + kPad <= cap[s]) return;
+    const size_t want = std::max(need, std::min(2 * cap[s], slot_bytes)) + kPad;
+    unsigned char* p = (unsigned char*)ds.alloc(want);
+    if (slot[s]) {
+      ds.copy(p, slot[s], len[s], ds.stream());
+      ds.release(slot[s]);
+    }
+    slot[s] = p;
+    cap[s] = want;
+  }
+  void put(int s, size_t off, const unsigned char* chunk, size_t n) override {
+    len[s] = off;
+    grow(s, off + n);
+    ds.copy(slot[s] + off, chunk, n, user_stream);
+    len[s] = off + n;
+  }
+  void carry(int from, size_t off, int to, size_t n) override {
+    len[to] = 0;
+    grow(to, n);
+    ds.copy(slot[to], slot[from] + off, n, ds.stream());
+    len[to] = n;
+  }
+  void stage(Engine& eng, int s, size_t n) override {
+    grow(s, n);
+    ds.zero(slot[s] + n, kPad);
+    eng.set_input_device(slot[s], n);
+  }
+  uint32_t checksum(Engine& eng, int s, size_t off, size_t n, int kind) override {
+    return eng.checksum_device(slot[s] + off, n, ds.stream(), kind);
+  }
+  void read(Engine& eng, int s, size_t off, size_t n, unsigned char* dst) override { eng.download(slot[s] + off, dst, n); }
+};
+
+WaveStaging* device_staging(int dev, void* stream) {
+  if (dev < 0 || dev >= Engine::device_count()) return nullptr;
+  return new DeviceWaveStaging(dev, stream);
+}
+
+// ZopfliB200CompressorNew (api.cpp) reaches device memory through these
+const bool g_registered = [] {
+  g_device_staging = device_staging;
+  g_pointer_device = Engine::pointer_device;
+  return true;
+}();
 
 }  // namespace
 

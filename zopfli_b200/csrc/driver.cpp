@@ -254,6 +254,17 @@ Schedule schedule(size_t nm, uint64_t device_memory) {
   return s;
 }
 
+}  // namespace
+
+// A call with master blocks for every pipeline runs nchunks x batch of them at once: one wave of a call on a
+// device with this much memory.
+size_t wave_master_blocks(uint64_t device_memory) {
+  const Schedule s = schedule(SIZE_MAX, device_memory);
+  return s.nchunks * s.batch;
+}
+
+namespace {
+
 // One deflate_units call with btype 2: the engine, its options, and the master blocks.  Every stage
 // below names the fields of Master it fills; the chunk pipelines work on disjoint master blocks.
 struct Call {

@@ -40,6 +40,14 @@ struct SpanPiece {
   bool final = false;
 };
 
+// ZopfliB200DeflateSpan's records of a range of master blocks: the driver's pieces, and the records made
+// of them (maximal runs of compressed pieces as bits, stored pieces as ranges of `stored`, their bytes).
+struct SpanRecords {
+  std::vector<Piece> pieces;
+  std::vector<SpanPiece> recs;
+  std::vector<unsigned char> stored;
+};
+
 struct HostTimes { double split = 0, emit = 0, other = 0; };
 extern HostTimes g_host_times;
 
@@ -53,6 +61,11 @@ bool debug_on();
 void deflate_units(Engine& eng, const ZopfliOptions* opt, int btype, bool final_last,
                    const std::vector<std::pair<size_t, size_t>>& units, size_t in_base,
                    std::vector<Piece>& pieces);
+
+// Master blocks that deflate_units runs at once on a device with this much memory (chunk pipelines x batch,
+// both from its schedule): the wave of a long ZopfliCompress call.  ZopfliB200Compressor asks for half the
+// device, so that its two waves in flight fit the budget of one call.
+size_t wave_master_blocks(uint64_t device_memory);
 
 // Places the pieces behind the caller's stream (bit phase *bp), emits them on the device and appends
 // the bytes to *out.  unit_bits (optional) receives the bit offset of every unit's first piece relative

@@ -628,8 +628,13 @@ Engine* Engine::acquire(int dev) {
   if (dev < 0) dev = default_device();
   std::unique_lock<std::mutex> lk(g_pool_mu);
   for (;;) {
-    for (size_t i = 0; i < g_free.size(); i++)
-      if (g_free[i]->device() == dev) { Engine* e = g_free[i]; g_free.erase(g_free.begin() + i); return e; }
+    // the free context created first: its arenas are already grown, so a process that makes one call at a time
+    // keeps using one context, and only calls that overlap grow others
+    for (Engine* e : g_all) {
+      if (e->device() != dev) continue;
+      auto f = std::find(g_free.begin(), g_free.end(), e);
+      if (f != g_free.end()) { g_free.erase(f); return e; }
+    }
     size_t have = 0;
     for (Engine* e : g_all) have += e->device() == dev;
     if (have < max_contexts()) {
@@ -1419,6 +1424,61 @@ void Engine::device_probe_parts(const uint32_t* hists, size_t n, uint32_t* smoot
   CK(cudaMemcpyAsync(tree_bits, d_tb, tb_b, cudaMemcpyDeviceToHost, l.stream));
   CK(cudaMemcpyAsync(dyn, d_dyn, dyn_b, cudaMemcpyDeviceToHost, l.stream));
   l.sync();
+}
+
+namespace {
+struct OnDevice {  // makes dev current for a scope, then restores the caller's device
+  int prev = 0;
+  explicit OnDevice(int dev) { CK(cudaGetDevice(&prev)); CK(cudaSetDevice(dev)); }
+  ~OnDevice() { cudaSetDevice(prev); }
+};
+}  // namespace
+
+DeviceStaging::DeviceStaging(int dev) : dev_(dev), stream_(nullptr), ev_(nullptr) {
+  OnDevice on(dev);
+  cudaStream_t s;
+  cudaEvent_t e;
+  CK(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
+  CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+  stream_ = s;
+  ev_ = e;
+}
+
+DeviceStaging::~DeviceStaging() {
+  OnDevice on(dev_);
+  CK(cudaStreamSynchronize((cudaStream_t)stream_));
+  CK(cudaEventDestroy((cudaEvent_t)ev_));
+  CK(cudaStreamDestroy((cudaStream_t)stream_));
+}
+
+void* DeviceStaging::alloc(size_t bytes) {
+  OnDevice on(dev_);
+  void* p = nullptr;
+  CK(cudaMallocAsync(&p, bytes, (cudaStream_t)stream_));
+  return p;
+}
+
+void DeviceStaging::release(void* p) {
+  if (!p) return;
+  OnDevice on(dev_);
+  CK(cudaFreeAsync(p, (cudaStream_t)stream_));
+}
+
+void DeviceStaging::copy(void* dst, const void* src, size_t n, void* user_stream) {
+  OnDevice on(dev_);
+  cudaStream_t s = (cudaStream_t)stream_;
+  if (user_stream != stream_) {  // the stream is non-blocking: it orders against the caller's only through an event
+    CK(cudaEventRecord((cudaEvent_t)ev_, (cudaStream_t)user_stream));
+    CK(cudaStreamWaitEvent(s, (cudaEvent_t)ev_, 0));
+  }
+  if (n) CK(cudaMemcpyAsync(dst, src, n, cudaMemcpyDeviceToDevice, s));
+  CK(cudaStreamSynchronize(s));
+}
+
+void DeviceStaging::zero(void* dst, size_t n) {
+  OnDevice on(dev_);
+  CK(cudaMemsetAsync(dst, 0, n, (cudaStream_t)stream_));
+  CK(cudaStreamSynchronize((cudaStream_t)stream_));
 }
 
 }  // namespace zb

@@ -168,4 +168,26 @@ class Engine {
   Impl* p_;
 };
 
+// Stream-ordered device memory of a caller that holds no engine context between its calls (the device
+// staging of ZopfliB200Compressor): allocations on a non-blocking stream of one device, and device-to-device
+// copies on it.  Every call leaves the calling thread's current device as it found it.
+class DeviceStaging {
+ public:
+  explicit DeviceStaging(int dev);
+  ~DeviceStaging();               // waits for the stream's work
+  void* alloc(size_t bytes);      // cudaMallocAsync on the stream
+  void release(void* p);          // cudaFreeAsync on the stream
+  // dst[0, n) <- src[0, n), ordered after the work queued on user_stream (a stream of this device, NULL = the
+  // legacy default stream; ignored when user_stream is this staging's own stream); blocks until the copy is done
+  void copy(void* dst, const void* src, size_t n, void* user_stream);
+  void zero(void* dst, size_t n);  // blocks until done
+  void* stream() const { return stream_; }
+  int device() const { return dev_; }
+
+ private:
+  int dev_;
+  void* stream_;
+  void* ev_;
+};
+
 }  // namespace zb
