@@ -143,9 +143,6 @@ __device__ __forceinline__ void sts_ring_if(uint32_t a, double c, uint32_t len, 
                "l"(__double_as_longlong(c)), "l"((long long)len), "r"((uint32_t)p)
                : "memory");
 }
-__device__ __forceinline__ void sts_f64_if(uint32_t a, double c, bool p) {
-  asm volatile("{ .reg .pred q; setp.ne.u32 q, %2, 0; @q st.shared.f64 [%0], %1; }" ::"r"(a), "d"(c), "r"((uint32_t)p) : "memory");
-}
 // (double)(float)x for 0 <= x < 3e38 outside the float-denormal range: round-to-nearest-even on
 // the 29 low mantissa bits, in integer arithmetic (keeps the conversion pipe off the cost chain)
 __device__ __forceinline__ double round_to_f32(double x) {
@@ -154,16 +151,6 @@ __device__ __forceinline__ double round_to_f32(double x) {
   b &= ~0x1FFFFFFFLL;
   return __longlong_as_double(b);
 }
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-#ifdef ZB_VAR_XCH_SPLIT
-#define ZB_XCH_LOAD(a, c, code) { (c) = lds_f64(a); (code) = lds_u32((a) + 8); }
-#define ZB_XCH_STORE(a, c, code, p) { sts_f64_if((a), (c), (p)); sts_u32_if((a) + 8, (code), (p)); }
-#else
-#define ZB_XCH_LOAD(a, c, code) lds_ring((a), (c), (code))
-#define ZB_XCH_STORE(a, c, code, p) sts_ring_if((a), (c), (code), (p))
-#endif
 __device__ __forceinline__ void mbar_arrive_a(uint32_t bar_a) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar_a) : "memory");
 }
@@ -188,12 +175,6 @@ __device__ __forceinline__ uint32_t lds_u16(uint32_t a) {
 __device__ __forceinline__ void sts_u16_if(uint32_t a, uint32_t v, bool p) {
   asm volatile("{ .reg .pred q; setp.ne.u32 q, %2, 0; @q st.shared.u16 [%0], %1; }" ::"r"(a), "h"((unsigned short)v), "r"((uint32_t)p) : "memory");
 }
-__device__ __forceinline__ void sts_f64(uint32_t a, double c) {
-  asm volatile("st.shared.f64 [%0], %1;" ::"r"(a), "d"(c) : "memory");
-}
-// The hand-off slot {cost, code} of the DP window.  Default: one 16-byte entry, LDS.128 / STS.128.
-// -DZB_VAR_XCH_SPLIT (experiment, off by default): 8 + 4 byte accesses at a + 0 / a + 8, which need no
-// aligned register quad (the 128-bit form costs a few register moves per step).
 __device__ __forceinline__ void sts_u32_if(uint32_t a, uint32_t v, bool p) {
   asm volatile("{ .reg .pred q; setp.ne.u32 q, %2, 0; @q st.shared.u32 [%0], %1; }" ::"r"(a), "r"(v), "r"((uint32_t)p) : "memory");
 }
@@ -592,14 +573,9 @@ __device__ uint64_t warp_dynamic_bits(const uint32_t* hist, CostStage& cs, uint3
   return 3 + (size1 < size0 ? size1 : size0);  // deflate.c:553-559
 }
 
-__device__ __forceinline__ uint32_t first_dist_of_symbol(int sd) {  // squeeze.c:176-179 table
-  return sd < 4 ? (uint32_t)sd + 1 : 1u + ((2u + (uint32_t)(sd & 1)) << (sd / 2 - 1));
-}
-
 // FollowPath (squeeze.c:338-389) of the traced symbols psym[cursor + t], t in [t0, t1), by one warp: store
 // entries t of cl / cd, histogram into `hist`.  128 symbols in flight per trip, fetched one trip ahead.
-// The wide form's slice of the loop the two-warp form runs inline over [0, nsym) (calling this function
-// there instead changes that kernel's register allocation).
+// The two-warp form runs it over [0, nsym), the wide form over one slice per warp.
 __device__ __forceinline__ void follow_path(const Batch& b, const SegDesc& sd, const uint8_t* in, const uint32_t* psym,
                                             uint32_t cursor, uint32_t t0, uint32_t t1, uint16_t* cl, uint16_t* cd,
                                             uint32_t* hist, uint32_t lane) {
@@ -632,22 +608,7 @@ __device__ __forceinline__ void follow_path(const Batch& b, const SegDesc& sd, c
       if (t >= t1) continue;
       const uint32_t len = e[u] & 511u;
       if (len >= (uint32_t)kMinMatch) {
-        const uint4 a = ra[u], c = rc[u];
-        uint32_t x = c.w;
-        if (c.w & kOverflowBit) {
-          x = 0;
-          if (len > run_len(c.z)) {
-            const uint32_t off = c.w & ~kOverflowBit, cnt = b.ovf[off];
-            for (uint32_t i = 0; i < cnt; i++) { uint32_t y = b.ovf[off + 1 + i]; if (run_len(y) >= len) { x = y; break; } }
-          }
-        }
-        if (len <= run_len(c.z)) x = c.z;
-        if (len <= run_len(c.y)) x = c.y;
-        if (len <= run_len(c.x)) x = c.x;
-        if (len <= run_len(a.w)) x = a.w;
-        if (len <= run_len(a.z)) x = a.z;
-        if (len <= run_len(a.y)) x = a.y;
-        if (len <= run_len(a.x)) x = a.x;
+        const uint32_t x = run_for_len(ra[u], rc[u], len, b.ovf);
         cl[t] = (uint16_t)len; cd[t] = (uint16_t)run_dist(x);
         atomicAdd(&hist[length_symbol((int)len)], 1u);
         atomicAdd(&hist[288 + run_dsym(x)], 1u);
@@ -1047,7 +1008,6 @@ __global__ void __launch_bounds__(NW * 32, NW == 2 ? 4 : 1) k_iterate(Batch b, c
       // was below 1e30 (not reachable with finite entropies)
       const int bl = bestlength, dsym = di == 0x7fffffff ? 0 : di;
       mincost = (double)(length_extra_bits(bl) + dist_symbol_extra_bits(dsym)) + s.lencost[bl < 3 ? 3 : bl] + s.dcost[dsym];
-      (void)first_dist_of_symbol;
     }
     // squeeze.c:293 skips an edge when costs[j+k] <= mincost + costs[j].  That is a pure
     // optimisation exactly when mincost <= every edge cost the model can produce (then
@@ -1144,7 +1104,7 @@ __global__ void __launch_bounds__(NW * 32, NW == 2 ? 4 : 1) k_iterate(Batch b, c
         const uint32_t ds3_ = lds_u8(dsx_s + (((U) + 3) * 32));                                             \
         const double llb2_ = lds_f64(gl_s + (((U) + 2) * 8));                                               \
         double en_c_; uint32_t en_l_;                                                                       \
-        ZB_XCH_LOAD(xch_r + ((((U) + 3) & 3) * 16), en_c_, en_l_);   /* pending(j+2), made at step j-1 */    \
+        lds_ring(xch_r + ((((U) + 3) & 3) * 16), en_c_, en_l_);   /* pending(j+2), made at step j-1 */       \
         double inc_ = kInfD; uint32_t inl_ = 0;                                                             \
         if (RING) { uint32_t fb_; lds_ring8(ring_s + (U) * 8, fb_, inl_); inc_ = (double)__uint_as_float(fb_);    \
                     sts_u32_if(ring_s + (U) * 8, kInfBits, is_l0); }                                         \
@@ -1162,7 +1122,7 @@ __global__ void __launch_bounds__(NW * 32, NW == 2 ? 4 : 1) k_iterate(Batch b, c
         w = ok_ ? rn_ : w;                                                                                  \
         wl = ok_ ? sidx : wl;                                                                               \
         const bool mine_ = lane_rot == (uint32_t)(U);   /* this lane's target is j+3: complete now */       \
-        ZB_XCH_STORE(xch_r + (((U) & 3) * 16), w, wl, mine_);                                               \
+        sts_ring_if(xch_r + (((U) & 3) * 16), w, wl, mine_);                                                \
         if (mine_) { w = inc_; wl = inl_; }                                                                 \
         sidx++;                                                                                             \
         e2c = en_c_; e2l = en_l_;                                                                           \
@@ -1335,7 +1295,7 @@ __global__ void __launch_bounds__(NW * 32, NW == 2 ? 4 : 1) k_iterate(Batch b, c
           }
           if (want_int && !imode) {  // every pending value the window holds must lie in the binade (or be infinite) to be carried over
             double xc; uint32_t xl;
-            ZB_XCH_LOAD(xch_r + ((j0 + 3u) & 3u) * 16, xc, xl);
+            lds_ring(xch_r + ((j0 + 3u) & 3u) * 16, xc, xl);
             (void)xl;
             want_int = __all_sync(0xffffffffu, !(w < i_lo_d) && !(e2c < i_lo_d) && !(xc < i_lo_d));
             if (want_int && j0 + 35 <= dirty_until) {  // so must every finite ring entry: it joins as an integer
@@ -1350,7 +1310,7 @@ __global__ void __launch_bounds__(NW * 32, NW == 2 ? 4 : 1) k_iterate(Batch b, c
           if (want_int) {
             wI = d2i(w, wl, t_l);
             e2I = d2i(e2c, e2l, j0 + 1u);
-            { double xc; uint32_t xl; ZB_XCH_LOAD(xch_r + xs * 16, xc, xl); const uint32_t xp = d2i(xc, xl, j0 + 2u); if (is_l0) dyn.xchi[xs] = xp; }
+            { double xc; uint32_t xl; lds_ring(xch_r + xs * 16, xc, xl); const uint32_t xp = d2i(xc, xl, j0 + 2u); if (is_l0) dyn.xchi[xs] = xp; }
             CJ = (__float_as_uint(__double2float_rn(cj)) - i_base) << 7;
             __syncwarp();
             tvI = lds_u32(ti_l + lds_u8(dsx_c) * 256 - 32 * 4);
@@ -1360,7 +1320,7 @@ __global__ void __launch_bounds__(NW * 32, NW == 2 ? 4 : 1) k_iterate(Batch b, c
           } else {
             i2d(wI, t_l, w, wl);
             i2d(e2I, j0 + 1u, e2c, e2l);
-            { double xc; uint32_t xl; i2d(lds_u32(xchi_r + xs * 4), j0 + 2u, xc, xl); ZB_XCH_STORE(xch_r + xs * 16, xc, xl, is_l0); }
+            { double xc; uint32_t xl; i2d(lds_u32(xchi_r + xs * 4), j0 + 2u, xc, xl); sts_ring_if(xch_r + xs * 16, xc, xl, is_l0); }
             cj = (double)__uint_as_float((CJ >> 7) + i_base);
             __syncwarp();
             tv = lds_f64(t0_l + lds_u8(dsx_c) * 512 - 32 * 8);
@@ -1399,31 +1359,12 @@ __global__ void __launch_bounds__(NW * 32, NW == 2 ? 4 : 1) k_iterate(Batch b, c
                 const uint32_t kend = ml < room ? ml : room;
                 const uint4* st4 = (const uint4*)&s.u.dp.runs[st][jl * kRunSlots];
                 const uint4 ea = st4[0], eb = st4[1];
-                const bool ovf = (eb.w & kOverflowBit) != 0;
                 const uint32_t cjb = i_base + (CJ >> 7);
-                // distance symbol of length k: first run whose end reaches k (overflow arena beyond eight runs)
-                auto run_of = [&](uint32_t k) -> uint32_t {
-                  uint32_t e = eb.w;
-                  if (ovf) {
-                    e = 0;
-                    if (k > run_len(eb.z)) {
-                      uint32_t off = eb.w & ~kOverflowBit, cnt = b.ovf[off];
-                      for (uint32_t r = 0; r < cnt; r++) { uint32_t x = b.ovf[off + 1 + r]; if (run_len(x) >= k) { e = x; break; } }
-                    }
-                  }
-                  if (k <= run_len(eb.z)) e = eb.z;
-                  if (k <= run_len(eb.y)) e = eb.y;
-                  if (k <= run_len(eb.x)) e = eb.x;
-                  if (k <= run_len(ea.w)) e = ea.w;
-                  if (k <= run_len(ea.z)) e = ea.z;
-                  if (k <= run_len(ea.y)) e = ea.y;
-                  if (k <= run_len(ea.x)) e = ea.x;
-                  return e;
-                };
                 for (uint32_t k = 35 + lane; k <= kend; k += 32) {
                   const uint32_t tga = ring_r + ((j + k - 3) & 511) * 8;
                   const uint32_t pendb = lds_u32(tga);
-                  const uint32_t E = lds_u32(tl_r + (((uint32_t)length_symbol((int)k) - 257u) * 32u + run_dsym(run_of(k))) * 4u);
+                  const uint32_t dsym = run_dsym(run_for_len(ea, eb, k, b.ovf));
+                  const uint32_t E = lds_u32(tl_r + (((uint32_t)length_symbol((int)k) - 257u) * 32u + dsym) * 4u);
                   const uint32_t rl = cjb + (E >> 1);
                   sts_ring8_if(tga, rl, kCodeLong | k, rl < pendb || (rl == pendb && (E & 1u) != 0));
                 }
@@ -1515,7 +1456,7 @@ __global__ void __launch_bounds__(NW * 32, NW == 2 ? 4 : 1) k_iterate(Batch b, c
             const uint32_t ds3 = lds_u8(dsx_c + (jl + 3) * 32);   // rows 32.. are the next stage (or its mirror)
             const double llb2 = lds_f64(gl_c + (jl + 2) * 8);
             double en_c; uint32_t en_l;
-            ZB_XCH_LOAD(xch_r + ((j + 3) & 3) * 16, en_c, en_l);  // pending(j+2), made at step j-1
+            lds_ring(xch_r + ((j + 3) & 3) * 16, en_c, en_l);  // pending(j+2), made at step j-1
             sts_u16_if(lac_c + jl * 2, lfin_prev, is_l0);
             const uint32_t m16 = lds_u16(mk_r + st * 64 + jl * 2);
             const uint32_t ml = m16 & 0x7fffu;
@@ -1551,23 +1492,8 @@ __global__ void __launch_bounds__(NW * 32, NW == 2 ? 4 : 1) k_iterate(Batch b, c
                 const uint32_t kend = ml < room ? ml : room;
                 const uint4* st4 = (const uint4*)&s.u.dp.runs[st][jl * kRunSlots];
                 const uint4 ea = st4[0], eb = st4[1];
-                const bool ovf = (eb.w & kOverflowBit) != 0;
                 for (uint32_t k = 35 + lane; k <= kend; k += 32) {
-                  uint32_t e = eb.w;
-                  if (ovf) {
-                    e = 0;
-                    if (k > run_len(eb.z)) {
-                      uint32_t off = eb.w & ~kOverflowBit, cnt = b.ovf[off];
-                      for (uint32_t r = 0; r < cnt; r++) { uint32_t x = b.ovf[off + 1 + r]; if (run_len(x) >= k) { e = x; break; } }
-                    }
-                  }
-                  if (k <= run_len(eb.z)) e = eb.z;
-                  if (k <= run_len(eb.y)) e = eb.y;
-                  if (k <= run_len(eb.x)) e = eb.x;
-                  if (k <= run_len(ea.w)) e = ea.w;
-                  if (k <= run_len(ea.z)) e = ea.z;
-                  if (k <= run_len(ea.y)) e = ea.y;
-                  if (k <= run_len(ea.x)) e = ea.x;
+                  const uint32_t e = run_for_len(ea, eb, k, b.ovf);
                   const uint32_t tga = ring_r + ((j + k - 3) & 511) * 8;
                   const double pend = (double)__uint_as_float(lds_u32(tga));
                   if (pend <= mc) continue;  // squeeze.c:293
@@ -1585,7 +1511,7 @@ __global__ void __launch_bounds__(NW * 32, NW == 2 ? 4 : 1) k_iterate(Batch b, c
             // target j+3 is complete for every length edge: hand it to the chain; its lane takes
             // on target j+35, whose ring entry (edges longer than 34) is complete as well
             const uint32_t src = (j + 3) & 31;
-            ZB_XCH_STORE(xch_r + (j & 3) * 16, w, wl, lane == src);
+            sts_ring_if(xch_r + (j & 3) * 16, w, wl, lane == src);
             double inc = kInfD; uint32_t inl = 0;
             __syncwarp();
             if (j + 35 <= dirty_until) {
@@ -1644,7 +1570,6 @@ __global__ void __launch_bounds__(NW * 32, NW == 2 ? 4 : 1) k_iterate(Batch b, c
       uint32_t idx = nb;  // current true path node
       const uint32_t la_a = smem_u32(&s.u.tr.la[0]), mk_a = smem_u32(&s.u.tr.mark[0]);
       const bool la_odd = (((uintptr_t)la) >> 1) & 1;  // make 4-byte loads aligned
-      constexpr uint32_t kSegLen = 128;
       while (idx > 0) {
         // window covers la[wlo .. idx], wlo chosen so that &la[wlo] is 4-byte aligned
         uint32_t wlo = idx >= 4088u ? idx - 4087u : 0u;
@@ -1666,21 +1591,15 @@ __global__ void __launch_bounds__(NW * 32, NW == 2 ? 4 : 1) k_iterate(Batch b, c
         }
         for (uint32_t t = lane; t < 2048; t += 32) ((uint32_t*)&s.u.tr.mark[0])[t] = 0;
         __syncwarp();
-        // one hop: length clamped to [1, i] so a corrupted chain cannot hang
-#define ZB_HOP(i_, l_) { asm volatile("ld.shared.u16 %0, [%1];" : "=r"(l_) : "r"(la_a + ((i_) - wlo) * 2)); l_ = max(l_, 1u); l_ = min(l_, (i_)); }
-        // ---- pass 1: speculative chains.  Segment s = positions (lo, hi], hi = idx - 128 s ----
-        const uint32_t hi = idx >= lane * kSegLen ? idx - lane * kSegLen : 0u;
-        const uint32_t lo = hi >= kSegLen ? hi - kSegLen : 0u;          // exclusive
-        const uint32_t floor_ = lo > wlo ? lo : (wlo > 0 ? wlo - 1 : 0u);  // stop below the window as well
-        uint32_t exit_s = hi, cnt_s = 0;
-        if (hi > 0 && hi >= wlo) {
-          uint32_t i = hi;
-          while (i > floor_) {
-            uint32_t l;
+        // ---- pass 1: speculative chains.  Lane s takes segment s = positions (lo, hi], hi = idx - 128 s ----
+        const TrSeg g = tr_seg(idx, wlo, lane);
+        uint32_t exit_s = g.hi, cnt_s = 0;
+        if (g.live) {
+          uint32_t i = g.hi;
+          while (i > g.floor_) {
             cnt_s++;
             asm volatile("st.shared.u16 [%0], %1;" ::"r"(mk_a + (i - wlo) * 2), "h"((unsigned short)cnt_s) : "memory");
-            ZB_HOP(i, l)
-            i -= l;
+            i -= tr_hop(la_a, wlo, i);
           }
           exit_s = i;
         }
@@ -1689,19 +1608,16 @@ __global__ void __launch_bounds__(NW * 32, NW == 2 ? 4 : 1) k_iterate(Batch b, c
         uint32_t e = idx;         // true node entering the current segment
         uint32_t my_from = 0xffffffffu, my_base = 0;  // this lane's chain is adopted from node number my_from on
         for (uint32_t sg = 0; sg < 32; sg++) {
-          const uint32_t shi = idx >= sg * kSegLen ? idx - sg * kSegLen : 0u;
-          if (shi == 0 || shi < wlo || e == 0 || e < wlo) break;
-          const uint32_t slo = shi >= kSegLen ? shi - kSegLen : 0u;
-          const uint32_t sfl = slo > wlo ? slo : (wlo > 0 ? wlo - 1 : 0u);
+          const TrSeg gs = tr_seg(idx, wlo, sg);
+          if (!gs.live || e == 0 || e < wlo) break;
           const uint32_t s_exit = __shfl_sync(0xffffffffu, exit_s, sg), s_cnt = __shfl_sync(0xffffffffu, cnt_s, sg);
-          if (e <= sfl) continue;  // the path jumps over this segment
+          if (e <= gs.floor_) continue;  // the path jumps over this segment
           uint32_t i = e, from = 0;
-          while (i > sfl) {
+          while (i > gs.floor_) {
             uint32_t mk;
             asm volatile("ld.shared.u16 %0, [%1];" : "=r"(mk) : "r"(mk_a + (i - wlo) * 2));
             if (mk) { from = mk; break; }
-            uint32_t l;
-            ZB_HOP(i, l)
+            const uint32_t l = tr_hop(la_a, wlo, i);
             i -= l;
             --cursor;
             if (lane == 0) psym[cursor] = (i << 9) | l;
@@ -1716,16 +1632,14 @@ __global__ void __launch_bounds__(NW * 32, NW == 2 ? 4 : 1) k_iterate(Batch b, c
         }
         // ---- pass 3: emit the adopted part of every chain ----
         if (my_from != 0xffffffffu) {
-          uint32_t i = hi, k = 0;
-          while (i > floor_) {
-            uint32_t l;
+          uint32_t i = g.hi, k = 0;
+          while (i > g.floor_) {
             k++;
-            ZB_HOP(i, l)
+            const uint32_t l = tr_hop(la_a, wlo, i);
             i -= l;
             if (k >= my_from) psym[my_base - 1 - (k - my_from)] = (i << 9) | l;
           }
         }
-#undef ZB_HOP
         idx = e;
         __syncwarp();
       }
@@ -1737,65 +1651,10 @@ __global__ void __launch_bounds__(NW * 32, NW == 2 ? 4 : 1) k_iterate(Batch b, c
     if constexpr (NW > 2) {
       wide_follow<NW>(W, s.hist, b, sd, in, psym, cursor, nsym);
     } else {
-    uint16_t* cl = b.st_ll[curbuf] + sd.pos_off;
-    uint16_t* cd = b.st_d[curbuf] + sd.pos_off;
-    for (int i = lane; i < 320; i += 32) s.hist[i] = 0;
-    __syncwarp();
-    uint32_t en[4];  // symbols of the next trip, fetched one trip ahead
-#pragma unroll
-    for (int u = 0; u < 4; u++) {
-      const uint32_t t = u * 32 + lane;
-      en[u] = t < nsym ? psym[cursor + t] : 1u;  // dummy literal at position 0 for the tail
-    }
-    for (uint32_t base = 0; base < nsym; base += 128) {
-      uint32_t e[4];
-      uint4 ra[4], rc[4];
-      uint32_t by[4];
-#pragma unroll
-      for (int u = 0; u < 4; u++) {
-        e[u] = en[u];
-        const uint32_t t = base + 128 + u * 32 + lane;
-        en[u] = t < nsym ? psym[cursor + t] : 1u;
-      }
-#pragma unroll
-      for (int u = 0; u < 4; u++) {
-        const uint32_t len = e[u] & 511u, pj = e[u] >> 9;
-        const uint4* r4 = (const uint4*)(b.runs + (sd.pos_off + pj) * kRunSlots);
-        if (len >= (uint32_t)kMinMatch) { ra[u] = r4[0]; rc[u] = r4[1]; by[u] = 0; }
-        else { ra[u] = make_uint4(0, 0, 0, 0); rc[u] = ra[u]; by[u] = in[pj]; }
-      }
-#pragma unroll
-      for (int u = 0; u < 4; u++) {
-        const uint32_t t = base + u * 32 + lane;
-        if (t >= nsym) continue;
-        const uint32_t len = e[u] & 511u;
-        if (len >= (uint32_t)kMinMatch) {
-          const uint4 a = ra[u], c = rc[u];
-          uint32_t x = c.w;
-          if (c.w & kOverflowBit) {
-            x = 0;
-            if (len > run_len(c.z)) {
-              const uint32_t off = c.w & ~kOverflowBit, cnt = b.ovf[off];
-              for (uint32_t i = 0; i < cnt; i++) { uint32_t y = b.ovf[off + 1 + i]; if (run_len(y) >= len) { x = y; break; } }
-            }
-          }
-          if (len <= run_len(c.z)) x = c.z;
-          if (len <= run_len(c.y)) x = c.y;
-          if (len <= run_len(c.x)) x = c.x;
-          if (len <= run_len(a.w)) x = a.w;
-          if (len <= run_len(a.z)) x = a.z;
-          if (len <= run_len(a.y)) x = a.y;
-          if (len <= run_len(a.x)) x = a.x;
-          cl[t] = (uint16_t)len; cd[t] = (uint16_t)run_dist(x);
-          atomicAdd(&s.hist[length_symbol((int)len)], 1u);
-          atomicAdd(&s.hist[288 + run_dsym(x)], 1u);
-        } else {
-          cl[t] = (uint16_t)by[u]; cd[t] = 0;
-          atomicAdd(&s.hist[by[u]], 1u);
-        }
-      }
-    }
-    __syncwarp();
+      for (int i = lane; i < 320; i += 32) s.hist[i] = 0;
+      __syncwarp();
+      follow_path(b, sd, in, psym, cursor, 0, nsym, b.st_ll[curbuf] + sd.pos_off, b.st_d[curbuf] + sd.pos_off, s.hist, lane);
+      __syncwarp();
     }
     ZB_TICK(3);
     if (fixed) { bestbuf = curbuf; best_size = nsym; bestcost = 0; it++; break; }

@@ -43,6 +43,30 @@ __host__ __device__ inline uint32_t run_len(uint32_t e) { return e & 511u; }
 __host__ __device__ inline uint32_t run_dist(uint32_t e) { return (e >> 9) & 32767u; }
 __host__ __device__ inline uint32_t run_dsym(uint32_t e) { return (e >> 24) & 31u; }
 
+// The run list of a parse position, as k_match writes it: entries in increasing len_end (and distance), entry r
+// covering the lengths above entry r-1's len_end, in eight slots a = slots 0-3, c = slots 4-7; unused slots are 0.
+// A position with more than eight entries keeps the first seven in slots 0-6 and kOverflowBit | off in slot 7,
+// and the overflow arena holds ovf[off] = count, then entries 7.. at ovf[off + 1 ..].
+// Returns the shortest-distance entry with len_end >= k (what FollowPath's limited search finds, squeeze.c:367).
+__device__ __forceinline__ uint32_t run_for_len(uint4 a, uint4 c, uint32_t k, const uint32_t* ovf) {
+  uint32_t e = c.w;
+  if (c.w & kOverflowBit) {
+    e = 0;
+    if (k > run_len(c.z)) {
+      const uint32_t off = c.w & ~kOverflowBit, cnt = ovf[off];
+      for (uint32_t i = 0; i < cnt; i++) { const uint32_t x = ovf[off + 1 + i]; if (run_len(x) >= k) { e = x; break; } }
+    }
+  }
+  if (k <= run_len(c.z)) e = c.z;
+  if (k <= run_len(c.y)) e = c.y;
+  if (k <= run_len(c.x)) e = c.x;
+  if (k <= run_len(a.w)) e = a.w;
+  if (k <= run_len(a.z)) e = a.z;
+  if (k <= run_len(a.y)) e = a.y;
+  if (k <= run_len(a.x)) e = a.x;
+  return e;
+}
+
 struct SegDesc {
   uint64_t instart, inend, winstart;  // absolute byte positions
   uint64_t key_off;   // element offset of this segment in hv/hv2/idx/rank arrays
@@ -590,32 +614,6 @@ __global__ void __launch_bounds__(kMatchWarps * 32) k_match(Batch b, const PosWo
     }
     __syncwarp();
   }
-}
-
-// distance of the shortest-distance match of length >= len at parse position (table lookup,
-// SURVEY App. A.3: this is what FollowPath's limited search returns, squeeze.c:367)
-__device__ __forceinline__ uint32_t table_dist(const Batch& b, uint64_t o, uint32_t len) {
-  const uint4* r4 = (const uint4*)(b.runs + o * kRunSlots);
-  const uint4 a = r4[0], c = r4[1];  // two independent 16-byte loads
-  uint32_t e = c.w;
-  if (c.w & kOverflowBit) {
-    e = 0;
-    if (len > run_len(c.z)) {
-      const uint32_t off = c.w & ~kOverflowBit, cnt = b.ovf[off];
-      for (uint32_t i = 0; i < cnt; i++) {
-        uint32_t x = b.ovf[off + 1 + i];
-        if (run_len(x) >= len) { e = x; break; }
-      }
-    }
-  }
-  if (len <= run_len(c.z)) e = c.z;
-  if (len <= run_len(c.y)) e = c.y;
-  if (len <= run_len(c.x)) e = c.x;
-  if (len <= run_len(a.w)) e = a.w;
-  if (len <= run_len(a.z)) e = a.z;
-  if (len <= run_len(a.y)) e = a.y;
-  if (len <= run_len(a.x)) e = a.x;
-  return run_dist(e);
 }
 
 // ---------------------------------------------------------------------------------------------
