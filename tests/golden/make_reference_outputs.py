@@ -16,7 +16,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 import zref  # noqa: E402
 
 MODULES = ["__graft_entry__", "bench", "test_gpu_parity", "test_gpu_parity_at_size", "test_gpu_integer_window",
-           "test_gpu_multi", "test_gpu_block_plan"]
+           "test_gpu_multi", "test_gpu_block_plan", "test_gpu_large_range"]
 
 
 def main(names):

@@ -463,6 +463,9 @@ struct Engine::Impl {
     L.segs.resize(r.size());
     for (size_t i = 0; i < r.size(); i++) {
       SegDesc& s = L.segs[i];
+      // a range of at most 0x7fff0000 bytes keeps npos and nkeys (range + 32 KiB) in the 32-bit counts of SegDesc,
+      // and every position and key index below 2^31 for the kernels' 32-bit index arithmetic (traced-path entries,
+      // position << 9 | length, are 64-bit for that reason)
       if (r[i].inend < r[i].instart || r[i].inend > insize || r[i].inend - r[i].instart > 0x7fff0000ull) {
         fprintf(stderr, "zopfli-b200: bad parse range [%llu,%llu) for input of %llu bytes\n",
                 (unsigned long long)r[i].instart, (unsigned long long)r[i].inend, (unsigned long long)insize);
@@ -494,6 +497,19 @@ struct Engine::Impl {
     });
   }
 
+  // capacity of the run-list overflow arena after a launch asked for `used` entries.  Slot 7 of a run list holds
+  // kOverflowBit | offset, so the arena stays within 2^31 entries.  The range guard of build_layout does not bound
+  // it (a position may ask for up to ~250 entries), so a batch that needs more is refused here rather than handed
+  // offsets that read the wrong entries.
+  static uint32_t grown_ovf_cap(uint64_t used) {
+    if (used >= kOverflowBit) {
+      fprintf(stderr, "zopfli-b200: the run lists of one batch need %llu overflow entries, more than 2^31\n",
+              (unsigned long long)used);
+      abort();
+    }
+    return (uint32_t)std::min<uint64_t>(used + used / 4 + 1024, kOverflowBit);
+  }
+
   // runs everything up to and including the match table on lane l; returns the Batch
   Batch prepare(const Layout& L, Lane& l) {
     const size_t ns = L.segs.size();
@@ -521,7 +537,7 @@ struct Engine::Impl {
       l.dsx.ensure(L.npos * 32 + 64);
       l.ovf.ensure((size_t)l.ovf_cap * 4);
       l.la.ensure((L.npos + ns) * 2 + 64);
-      l.path.ensure((L.npos + ns) * 4 + 64);
+      l.path.ensure((L.npos + ns) * 8 + 64);
       { std::lock_guard<std::mutex> g(mu); ensure_log(); }
     }
     Batch b;
@@ -544,10 +560,10 @@ struct Engine::Impl {
     b.runs = l.runs.as<uint32_t>();
     b.dsx = l.dsx.as<uint8_t>();
     b.ovf = l.ovf.as<uint32_t>();
-    b.ovf_used = l.counters.as<uint32_t>();
+    b.ovf_used = &l.counters.as<Counters>()->ovf_used;
     b.ovf_cap = l.ovf_cap;
     b.la = l.la.as<uint16_t>();
-    b.path = l.path.as<uint32_t>();
+    b.path = l.path.as<uint64_t>();
     b.st_ll[0] = l.st[0].as<uint16_t>();
     b.st_d[0] = l.st[1].as<uint16_t>();
     b.st_ll[1] = l.st[2].as<uint16_t>();
@@ -559,7 +575,7 @@ struct Engine::Impl {
     b.logtab_n = logtab_n;
     b.out_ll = l.out_ll.as<uint16_t>();
     b.out_d = l.out_d.as<uint16_t>();
-    b.out_used = l.counters.as<uint32_t>() + 1;
+    b.out_used = &l.counters.as<Counters>()->out_used;
     static const uint32_t dp_flags = [] { const char* e = getenv("ZOPFLI_B200_INTDP"); return (e && atoi(e) == 0) ? 0u : 1u; }();
     b.dp_flags = dp_flags;
 
@@ -865,7 +881,7 @@ void Engine::parse_common(const std::vector<ParseRange>& ranges, ParseResult& ou
   Impl::Layout L;
   m.build_layout(ranges, L);
   std::vector<JobState> js(ns);
-  uint32_t counters[2] = {0, 0};
+  Counters counters{};
   {  // statistics counts stay below 2 x symbols (blended statistics, squeeze.c:70-75): size the log table for it
     uint64_t need = 0;
     for (const SegDesc& sg : L.segs)
@@ -930,19 +946,19 @@ void Engine::parse_common(const std::vector<ParseRange>& ranges, ParseResult& ou
     l.acc.launches++;
     l.tic();
     CK(cudaMemcpyAsync(js.data(), l.jobs.p, ns * sizeof(JobState), cudaMemcpyDeviceToHost, l.stream));
-    CK(cudaMemcpyAsync(counters, l.counters.p, sizeof(counters), cudaMemcpyDeviceToHost, l.stream));
+    CK(cudaMemcpyAsync(&counters, l.counters.p, sizeof(counters), cudaMemcpyDeviceToHost, l.stream));
     if (it_stride) {
       iter_costs->assign((size_t)ns * it_stride, ~0ull);
       CK(cudaMemcpyAsync(iter_costs->data(), l.iterc.p, (size_t)ns * it_stride * 8, cudaMemcpyDeviceToHost, l.stream));
     }
     l.toc(l.acc.ms_d2h);
     l.sync();
-    if (L.any_parse && counters[0] > l.ovf_cap) {  // run-list overflow arena too small: grow, redo
-      l.ovf_cap = counters[0] + counters[0] / 4 + 1024;
+    if (L.any_parse && counters.ovf_used > l.ovf_cap) {  // run-list overflow arena too small: grow, redo
+      l.ovf_cap = Impl::grown_ovf_cap(counters.ovf_used);
       if (attempt > 2) { fprintf(stderr, "zopfli-b200: overflow arena did not converge\n"); abort(); }
       continue;
     }
-    const uint32_t total = dest < 0 ? counters[1] : 0u;
+    const uint32_t total = dest < 0 ? counters.out_used : 0u;
     out.ll.resize(total);
     out.d.resize(total);
     if (total) {
@@ -1003,10 +1019,11 @@ void Engine::match_table(uint64_t instart, uint64_t inend, std::vector<uint16_t>
   const size_t n = (size_t)(inend - instart);
   for (int attempt = 0;; attempt++) {
     m.prepare(L, l);
-    uint32_t used = 0;
-    CK(cudaMemcpyAsync(&used, l.counters.p, 4, cudaMemcpyDeviceToHost, l.stream));
+    Counters c{};
+    CK(cudaMemcpyAsync(&c, l.counters.p, sizeof(c), cudaMemcpyDeviceToHost, l.stream));
     l.sync();
-    if (used > l.ovf_cap) { l.ovf_cap = used + used / 4 + 1024; if (attempt > 2) abort(); continue; }
+    const size_t used = c.ovf_used;
+    if (used > l.ovf_cap) { l.ovf_cap = Impl::grown_ovf_cap(used); if (attempt > 2) abort(); continue; }
     h_ld.resize(n); h_runs.resize(n * kRunSlots); h_mlen.resize(n); h_ovf.resize(used + 1);
     h_hv.resize(L.nkeys); h_hv2.resize(L.nkeys); h_same.resize(n);
     if (n) {

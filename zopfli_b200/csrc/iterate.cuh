@@ -576,17 +576,17 @@ __device__ uint64_t warp_dynamic_bits(const uint32_t* hist, CostStage& cs, uint3
 // FollowPath (squeeze.c:338-389) of the traced symbols psym[cursor + t], t in [t0, t1), by one warp: store
 // entries t of cl / cd, histogram into `hist`.  128 symbols in flight per trip, fetched one trip ahead.
 // The two-warp form runs it over [0, nsym), the wide form over one slice per warp.
-__device__ __forceinline__ void follow_path(const Batch& b, const SegDesc& sd, const uint8_t* in, const uint32_t* psym,
+__device__ __forceinline__ void follow_path(const Batch& b, const SegDesc& sd, const uint8_t* in, const uint64_t* psym,
                                             uint32_t cursor, uint32_t t0, uint32_t t1, uint16_t* cl, uint16_t* cd,
                                             uint32_t* hist, uint32_t lane) {
-  uint32_t en[4];  // symbols of the next trip, fetched one trip ahead
+  uint64_t en[4];  // symbols of the next trip, fetched one trip ahead
 #pragma unroll
   for (int u = 0; u < 4; u++) {
     const uint32_t t = t0 + u * 32 + lane;
     en[u] = t < t1 ? psym[cursor + t] : 1u;  // dummy literal at position 0 for the tail
   }
   for (uint32_t base = t0; base < t1; base += 128) {
-    uint32_t e[4];
+    uint64_t e[4];
     uint4 ra[4], rc[4];
     uint32_t by[4];
 #pragma unroll
@@ -597,7 +597,7 @@ __device__ __forceinline__ void follow_path(const Batch& b, const SegDesc& sd, c
     }
 #pragma unroll
     for (int u = 0; u < 4; u++) {
-      const uint32_t len = e[u] & 511u, pj = e[u] >> 9;
+      const uint32_t len = (uint32_t)e[u] & 511u, pj = (uint32_t)(e[u] >> 9);
       const uint4* r4 = (const uint4*)(b.runs + (sd.pos_off + pj) * kRunSlots);
       if (len >= (uint32_t)kMinMatch) { ra[u] = r4[0]; rc[u] = r4[1]; by[u] = 0; }
       else { ra[u] = make_uint4(0, 0, 0, 0); rc[u] = ra[u]; by[u] = in[pj]; }
@@ -606,7 +606,7 @@ __device__ __forceinline__ void follow_path(const Batch& b, const SegDesc& sd, c
     for (int u = 0; u < 4; u++) {
       const uint32_t t = base + u * 32 + lane;
       if (t >= t1) continue;
-      const uint32_t len = e[u] & 511u;
+      const uint32_t len = (uint32_t)e[u] & 511u;
       if (len >= (uint32_t)kMinMatch) {
         const uint32_t x = run_for_len(ra[u], rc[u], len, b.ovf);
         cl[t] = (uint16_t)len; cd[t] = (uint16_t)run_dist(x);
@@ -679,7 +679,7 @@ __device__ __forceinline__ uint32_t tr_walk(uint32_t la_a, uint32_t mk_a, uint32
 //   pass 3  every segment writes its symbols at their offset in psym.
 // psym[cursor .. nb] comes out as (start position << 9 | length) of the path, in order.  Returns cursor.
 template <int NW>
-__device__ __noinline__ uint32_t wide_trace(WideSmem<NW>& W, const uint16_t* la, uint32_t* psym, uint32_t nb) {
+__device__ __noinline__ uint32_t wide_trace(WideSmem<NW>& W, const uint16_t* la, uint64_t* psym, uint32_t nb) {
   constexpr uint32_t kSeg = WideSmem<NW>::kSeg, kWin = WideSmem<NW>::kWin, NT = NW * 32;
   const uint32_t s = threadIdx.x, lane = s & 31u, full = 0xffffffffu;
   const uint32_t la_a = smem_u32(&W.la[0]), mk_a = smem_u32(&W.mark[0]);
@@ -775,7 +775,7 @@ __device__ __noinline__ uint32_t wide_trace(WideSmem<NW>& W, const uint16_t* la,
       for (uint32_t k = 0; k < n; k++) {
         const uint32_t l = tr_hop(la_a, wlo, i);
         i -= l;
-        psym[top - 1 - k] = (i << 9) | l;
+        psym[top - 1 - k] = ((uint64_t)i << 9) | l;
       }
     }
     idx = nidx;
@@ -789,7 +789,7 @@ __device__ __noinline__ uint32_t wide_trace(WideSmem<NW>& W, const uint16_t* la,
 // histogram of its own; warp 0 adds them up into s.hist (integer sums: exact in any order)
 template <int NW>
 __device__ __noinline__ void wide_follow(WideSmem<NW>& W, uint32_t* hist_out, const Batch& b, const SegDesc& sd,
-                                         const uint8_t* in, const uint32_t* psym, uint32_t cursor, uint32_t nsym) {
+                                         const uint8_t* in, const uint64_t* psym, uint32_t cursor, uint32_t nsym) {
   const uint32_t lane = threadIdx.x & 31u, wid = threadIdx.x >> 5;
   const int cb = (int)W.curbuf;
   uint32_t* h = W.hist[wid];
@@ -835,7 +835,7 @@ __global__ void __launch_bounds__(NW * 32, NW == 2 ? 4 : 1) k_iterate(Batch b, c
     return;
   }
   uint16_t* la = b.la + sd.pos_off + seg;
-  uint32_t* psym = b.path + sd.pos_off + seg;  // traced symbols: (start position << 9) | length
+  uint64_t* psym = b.path + sd.pos_off + seg;  // traced symbols: (start position << 9) | length
   const uint8_t* in = b.in + sd.instart;
   const uint16_t* mlen = b.mlen + sd.pos_off;
   const uint32_t* runs_g = b.runs + sd.pos_off * kRunSlots;
@@ -1620,7 +1620,7 @@ __global__ void __launch_bounds__(NW * 32, NW == 2 ? 4 : 1) k_iterate(Batch b, c
             const uint32_t l = tr_hop(la_a, wlo, i);
             i -= l;
             --cursor;
-            if (lane == 0) psym[cursor] = (i << 9) | l;
+            if (lane == 0) psym[cursor] = ((uint64_t)i << 9) | l;
           }
           if (from) {  // merged: nodes from..s_cnt of lane sg's chain are on the path
             if (lane == sg) { my_from = from; my_base = cursor; }
@@ -1637,7 +1637,7 @@ __global__ void __launch_bounds__(NW * 32, NW == 2 ? 4 : 1) k_iterate(Batch b, c
             k++;
             const uint32_t l = tr_hop(la_a, wlo, i);
             i -= l;
-            if (k >= my_from) psym[my_base - 1 - (k - my_from)] = (i << 9) | l;
+            if (k >= my_from) psym[my_base - 1 - (k - my_from)] = ((uint64_t)i << 9) | l;
           }
         }
         idx = e;

@@ -92,6 +92,13 @@ struct JobState {   // per segment, written by k_greedy / k_iterate
   uint32_t dpn[6];       // groups of each kind; [5] = positions that went through the per-step general loop
 };
 
+struct Counters {                // per batch, zeroed before its launches
+  unsigned long long ovf_used;   // overflow-arena entries k_match asked for, including those that did not fit (64 bits:
+                                 // a batch may ask for more than 2^32, and a wrapped count would hand out used offsets)
+  uint32_t out_used;             // symbols of the packed results (k_pack)
+  uint32_t pad_;
+};
+
 struct Batch {
   const uint8_t* in;        // whole input (device), padded by >= 16 readable bytes
   uint64_t insize;
@@ -116,11 +123,12 @@ struct Batch {
                     // kNoEdge if 3+l exceeds the longest match / the block end (the DP's 32-wide
                     // register window works on these)
   uint32_t* ovf;    // overflow arena: [count, entries...]
-  uint32_t* ovf_used;
-  uint32_t ovf_cap;
+  unsigned long long* ovf_used;  // Counters::ovf_used
+  uint32_t ovf_cap;              // <= 2^31: slot 7 of a run list holds kOverflowBit | offset
   // parse state
   uint16_t* la;     // [npos + nsegs] length_array, nb+1 per segment (offset pos_off + seg)
-  uint32_t* path;   // [npos + nsegs] traced symbols (start position << 9 | length), filled from the end
+  uint64_t* path;   // [npos + nsegs] traced symbols (start position << 9 | length), filled from the end; 64 bits
+                    // because a block may hold more than 2^23 positions (build_layout accepts up to 0x7fff0000)
   uint16_t* st_ll[3];
   uint16_t* st_d[3];
   JobState* jobs;
@@ -129,7 +137,7 @@ struct Batch {
   // packed results
   uint16_t* out_ll;
   uint16_t* out_d;
-  uint32_t* out_used;
+  uint32_t* out_used;       // Counters::out_used
   // verbose: cost of every iteration of every block (squeeze.c:492-495), [nsegs][iter_stride]; null otherwise
   uint64_t* iter_cost;
   uint32_t iter_stride;
@@ -599,7 +607,9 @@ __global__ void __launch_bounds__(kMatchWarps * 32) k_match(Batch b, const PosWo
       } else {
         uint32_t off = 0;
         uint32_t extra = nruns - (kRunSlots - 1);
-        if (lane == 0) off = atomicAdd(b.ovf_used, extra + 1);
+        // an offset past the end of the arena is clamped to it: these entries do not fit, and ovf_used > ovf_cap
+        // makes the host grow the arena and redo the batch
+        if (lane == 0) off = (uint32_t)min(atomicAdd(b.ovf_used, (unsigned long long)(extra + 1)), (unsigned long long)b.ovf_cap);
         off = __shfl_sync(0xffffffffu, off, 0);
         if (off + extra + 1 <= b.ovf_cap) {
           if (lane == 0) b.ovf[off] = extra;
