@@ -240,12 +240,14 @@ void ZopfliB200DistPlacement(const uint64_t* len8, int world, unsigned phase0, u
 /* CRC-32 of the gzip trailer (gzip_container.c:27-81) and its combination across shards. */
 uint32_t ZopfliB200Crc32(const unsigned char* data, size_t size);
 uint32_t ZopfliB200Crc32Combine(uint32_t crc1, uint32_t crc2, uint64_t len2);
-/* Adler-32 of the zlib trailer (zlib_container.c:29-48), threaded with an exact combination, and the
- * combination of consecutive slices (adler32 of A|B from those of A and B and |B|). */
+/* Adler-32 of the zlib trailer (zlib_container.c:29-48), computed as ZopfliB200Crc32 is (from 4 MiB on, one
+ * slice per host thread, the slices combined exactly), and the combination of consecutive slices (adler32
+ * of A|B from those of A and B and |B|). */
 uint32_t ZopfliB200Adler32(const unsigned char* data, size_t size);
 uint32_t ZopfliB200Adler32Combine(uint32_t adler1, uint32_t adler2, uint64_t len2);
-/* The slice algebra of the device checksums (csrc/checksum.hpp) run on the host: the input cut into
- * slices of slice_bytes, each reduced on its own and combined.  kind 0: CRC-32, 1: Adler-32. */
+/* The host checksum behind ZopfliB200Crc32, ZopfliB200Adler32 and the gzip / zlib trailers, run at a chosen
+ * slice size: the input cut into slices of slice_bytes (0 counts as 1), reduced side by side and combined
+ * with the slice algebra of the device checksums (csrc/checksum.hpp).  kind 0: CRC-32, 1: Adler-32. */
 uint32_t ZopfliB200HostChecksumSliced(const unsigned char* data, size_t size, size_t slice_bytes, int kind);
 
 /* Engine control / introspection. */

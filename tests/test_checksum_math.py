@@ -1,7 +1,8 @@
-"""The slice algebra behind the device CRC-32 / Adler-32 (zopfli_b200/csrc/checksum.hpp), run on the host
-through ZopfliB200HostChecksumSliced: the input is cut into slices that are reduced one by one and
-combined, and the result must be zlib's for every length and slice size.  Runs without a GPU, in both the
-product library and the host-mock build of the same sources."""
+"""The production host checksum (host_checksum in zopfli_b200/csrc/api.cpp, the slice algebra of
+checksum.hpp that the device CRC-32 / Adler-32 also use) at a chosen slice size, through
+ZopfliB200HostChecksumSliced: the input is cut into slices that are reduced side by side and combined, and
+the result must be zlib's for every length and slice size.  Runs without a GPU, in both the product library
+and the host-mock build of the same sources."""
 import ctypes as C
 import os
 import subprocess

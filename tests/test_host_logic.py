@@ -342,7 +342,8 @@ def test_optimize_for_rle_restatement(ref, host):
 
 def test_checksums_threaded_and_combined(mock):
     """CRC-32 / Adler-32 of the container trailers (gzip_container.c:27-81, zlib_container.c:29-48): the
-    threaded versions with their exact combination rules against zlib, across the threading threshold."""
+    host checksum at its default slicing (one slice per host thread from 4 MiB on) against zlib, across
+    that threshold."""
     import zlib
     rng = np.random.default_rng(8)
     for n in (0, 1, 5551, 5553, 70000, (4 << 20) - 1, (4 << 20) + 12345, 9000001):

@@ -484,7 +484,7 @@ class Library:
         return int(self.lib.ZopfliB200Adler32Combine(adler1, adler2, len2))
 
     def host_checksum_sliced(self, data: bytes, slice_bytes: int, kind: int) -> int:
-        """the device checksums' slice algebra on the host; kind 0 CRC-32, 1 Adler-32"""
+        """the production host checksum at slices of slice_bytes; kind 0 CRC-32, 1 Adler-32"""
         a = _pad(data)
         return int(self.lib.ZopfliB200HostChecksumSliced(a.ctypes.data, len(data), slice_bytes, kind))
 

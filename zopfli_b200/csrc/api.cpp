@@ -43,6 +43,11 @@ void api_call_done(std::vector<uint64_t>& layout, double t0) {
   g_total_ms += now_ms() - t0;
 }
 
+int trailer_kind(ZopfliFormat fmt) {
+  if (fmt != ZOPFLI_FORMAT_GZIP && fmt != ZOPFLI_FORMAT_ZLIB && fmt != ZOPFLI_FORMAT_DEFLATE) return -1;
+  return fmt == ZOPFLI_FORMAT_GZIP ? kCkCrc32 : (fmt == ZOPFLI_FORMAT_ZLIB ? kCkAdler32 : kCkNone);
+}
+
 // header bytes of the gzip (gzip_container.c:95-104) or zlib (zlib_container.c:58-64) container; 0 for raw deflate
 int container_header(ZopfliFormat fmt, unsigned char* hdr) {
   if (fmt == ZOPFLI_FORMAT_GZIP) {
@@ -60,7 +65,9 @@ int container_header(ZopfliFormat fmt, unsigned char* hdr) {
   return 0;
 }
 
-void report_size(ZopfliFormat fmt, size_t insize, size_t outsize) {
+// the verbose report after the deflate body (fmt DEFLATE, outsize = its bytes) or after the gzip / zlib
+// container (outsize = the whole output buffer)
+static void report_size(ZopfliFormat fmt, size_t insize, size_t outsize) {
   const double removed = 100.0 * (double)(insize - outsize) / (double)insize;
   if (fmt == ZOPFLI_FORMAT_DEFLATE)  // deflate.c:925-928
     fprintf(stderr, "Original Size: %lu, Deflate: %lu, Compression: %f%% Removed\n", (unsigned long)insize,
@@ -68,6 +75,11 @@ void report_size(ZopfliFormat fmt, size_t insize, size_t outsize) {
   else  // gzip_container.c:118-122, zlib_container.c:73-77
     fprintf(stderr, "Original Size: %d, %s: %d, Compression: %f%% Removed\n", (int)insize,
             fmt == ZOPFLI_FORMAT_GZIP ? "Gzip" : "Zlib", (int)outsize, removed);
+}
+
+void report_sizes(ZopfliFormat fmt, size_t insize, size_t deflate_bytes, size_t outsize) {
+  report_size(ZOPFLI_FORMAT_DEFLATE, insize, deflate_bytes);
+  if (fmt != ZOPFLI_FORMAT_DEFLATE) report_size(fmt, insize, outsize);
 }
 
 bool seam_pieces(size_t insize, const unsigned short* ll, const unsigned short* d, size_t n, size_t npieces,
@@ -161,81 +173,51 @@ void deflate_span_records(Engine& eng, const ZopfliOptions* opt, size_t base, si
 
 namespace {
 
-// ---- CRC-32 (gzip_container.c:27-81 computes the same polynomial bytewise): slicing-by-8 ----
-uint32_t g_crc_tab[8][256];
-std::once_flag g_crc_once;
-void crc_fill() {
-  for (uint32_t i = 0; i < 256; i++) g_crc_tab[0][i] = crc_table_entry(0, i);
-  for (uint32_t i = 0; i < 256; i++)
-    for (int t = 1; t < 8; t++) g_crc_tab[t][i] = (g_crc_tab[t - 1][i] >> 8) ^ g_crc_tab[0][g_crc_tab[t - 1][i] & 255];
-}
-void crc_init() { std::call_once(g_crc_once, crc_fill); }
-uint32_t crc32_range(const unsigned char* p, size_t n, uint32_t crc) {  // crc is the running (inverted) state
-  while (n && ((uintptr_t)p & 7)) { crc = g_crc_tab[0][(crc ^ *p++) & 255] ^ (crc >> 8); n--; }
-  while (n >= 8) {
-    uint64_t v;
-    memcpy(&v, p, 8);
-    uint32_t lo = (uint32_t)v ^ crc, hi = (uint32_t)(v >> 32);
-    crc = g_crc_tab[7][lo & 255] ^ g_crc_tab[6][(lo >> 8) & 255] ^ g_crc_tab[5][(lo >> 16) & 255] ^
-          g_crc_tab[4][lo >> 24] ^ g_crc_tab[3][hi & 255] ^ g_crc_tab[2][(hi >> 8) & 255] ^
-          g_crc_tab[1][(hi >> 16) & 255] ^ g_crc_tab[0][hi >> 24];
-    p += 8;
-    n -= 8;
+// ---- CRC-32 (gzip_container.c:27-81) and Adler-32 (zlib_container.c:29-48) of host bytes ----
+// The input is cut into slices of `slice` bytes (0: one slice per host thread from 4 MiB on, else a single
+// slice).  The slices are reduced side by side and combined with the slice algebra of checksum.hpp, as the
+// device kernels combine theirs.
+uint32_t host_checksum(const unsigned char* d, size_t n, int kind, size_t slice) {
+  static const struct CrcTables {
+    uint32_t t[8][256];
+    CrcTables() {
+      for (int k = 0; k < 8; k++)
+        for (uint32_t i = 0; i < 256; i++) t[k][i] = crc_table_entry(k, i);
+    }
+  } T;
+  static const CrcShiftTable sh = crc_shift_table();
+  if (slice == 0) {
+    const size_t nt = n >= (4u << 20) ? (size_t)host_threads() : 1;
+    slice = std::max<size_t>((n + nt - 1) / nt, 1);
   }
-  while (n--) crc = g_crc_tab[0][(crc ^ *p++) & 255] ^ (crc >> 8);
-  return crc;
-}
-uint32_t crc32_parallel(const unsigned char* p, size_t n) {
-  crc_init();
-  unsigned nt = std::thread::hardware_concurrency();
-  if (nt < 1) nt = 1;
-  if (nt > 16) nt = 16;
-  if (n < (4u << 20) || nt == 1) return crc32_range(p, n, 0xffffffffu) ^ 0xffffffffu;
-  std::vector<uint32_t> part(nt);
-  std::vector<std::thread> th;
-  size_t chunk = (n + nt - 1) / nt;
-  for (unsigned t = 0; t < nt; t++)
-    th.emplace_back([&, t] {
-      size_t a = t * chunk, b = a + chunk > n ? n : a + chunk;
-      part[t] = a < b ? (crc32_range(p + a, b - a, 0xffffffffu) ^ 0xffffffffu) : 0;
-    });
-  for (auto& t : th) t.join();
-  uint32_t crc = part[0];
-  for (unsigned t = 1; t < nt; t++) {
-    size_t a = t * chunk, b = a + chunk > n ? n : a + chunk;
-    if (a < b) crc = crc32_combine(crc, part[t], b - a);
+  std::vector<ChecksumAcc> part((n + slice - 1) / slice);
+  parallel_for(part.size(), [&](size_t s) {
+    const unsigned char* p = d + s * slice;
+    const size_t len = std::min(slice, n - s * slice), after = n - s * slice - len;
+    if (kind == kCkCrc32) {  // slicing-by-8 from register 0, then past the bytes after the slice
+      uint32_t c = 0;
+      size_t k = 0;
+      for (; k < len && ((uintptr_t)(p + k) & 7); k++) c = T.t[0][(c ^ p[k]) & 255] ^ (c >> 8);
+      for (; k + 8 <= len; k += 8) {
+        uint64_t v;
+        memcpy(&v, p + k, 8);
+        c = crc_slice8(c, (uint32_t)v, (uint32_t)(v >> 32), T.t);
+      }
+      for (; k < len; k++) c = T.t[0][(c ^ p[k]) & 255] ^ (c >> 8);
+      part[s].crc0 = crc_shift(c, after, sh);
+    } else {
+      const AdlerPart q = adler_chunk(p, len);
+      part[s].a = q.s1;
+      part[s].b = (q.s2 + (after % kAdlerMod) * q.s1) % kAdlerMod;
+    }
+  });
+  ChecksumAcc acc = {0, 0, 0, 0};
+  for (const ChecksumAcc& q : part) {
+    acc.crc0 ^= q.crc0;
+    acc.a += q.a;
+    acc.b += q.b;
   }
-  return crc;
-}
-
-// ---- Adler-32 (zlib_container.c:29-48 computes it serially) ----
-// s1 = 1 + sum(d_i), s2 = sum over i of s1 after byte i (both mod 65521).  Sums of byte values and of
-// position-weighted byte values are associative, so chunks (adler_chunk, checksum.hpp) are summed by
-// threads and combined below.
-uint32_t adler32(const unsigned char* data, size_t size) {
-  unsigned nt = std::thread::hardware_concurrency();
-  if (nt < 1) nt = 1;
-  if (nt > 16) nt = 16;
-  if (size < (4u << 20)) nt = 1;
-  std::vector<AdlerPart> part(nt);
-  const size_t chunk = (size + nt - 1) / nt;
-  std::vector<std::thread> th;
-  for (unsigned t = 1; t < nt; t++)
-    th.emplace_back([&, t] {
-      const size_t a = std::min(size, t * chunk), b = std::min(size, a + chunk);
-      part[t] = adler_chunk(data + a, b - a);
-    });
-  part[0] = adler_chunk(data, std::min(size, chunk));
-  for (auto& t : th) t.join();
-  // with a = sum of bytes and b = sum of prefix sums (both without the initial 1):
-  //   a(A|B) = a(A) + a(B),  b(A|B) = b(A) + len(B) * a(A) + b(B);  the initial s1 = 1 adds `size` to s2
-  uint64_t a = 0, b = 0;
-  for (unsigned t = 0; t < nt; t++) {
-    b = (b + (part[t].len % 65521) * a + part[t].s2) % 65521;
-    a = (a + part[t].s1) % 65521;
-  }
-  const uint64_t s1 = (1 + a) % 65521, s2 = (b + size % 65521) % 65521;
-  return (uint32_t)((s2 << 16) | s1);
+  return kind == kCkCrc32 ? crc_finish(acc.crc0, n, sh) : adler_finish(acc.a, acc.b, n);
 }
 
 void deflate_impl(const ZopfliOptions* options, int btype, int final, const unsigned char* in,
@@ -269,31 +251,19 @@ void deflate_impl(const ZopfliOptions* options, int btype, int final, const unsi
 // the containers (gzip_container.c:84-124, zlib_container.c:50-79) around a deflate body produced by `body`
 template <typename Body>
 void container_impl(const ZopfliOptions* options, ZopfliFormat fmt, const unsigned char* in, size_t insize,
-                    unsigned char** out, size_t* outsize, Body deflate_impl_fn);
-
-void compress_impl(const ZopfliOptions* options, ZopfliFormat fmt, const unsigned char* in, size_t insize,
-                   const unsigned char* dev_in, unsigned char** out, size_t* outsize) {
-  container_impl(options, fmt, in, insize, out, outsize, [&](unsigned char* bp) {
-    deflate_impl(options, 2, 1, in, insize, dev_in, bp, out, outsize);
-  });
-}
-
-template <typename Body>
-void container_impl(const ZopfliOptions* options, ZopfliFormat fmt, const unsigned char* in, size_t insize,
                     unsigned char** out, size_t* outsize, Body body) {
-  unsigned char bp = 0;
-  if (fmt == ZOPFLI_FORMAT_DEFLATE) {
-    body(&bp);
-    return;
-  }
-  if (fmt != ZOPFLI_FORMAT_GZIP && fmt != ZOPFLI_FORMAT_ZLIB) {
+  const int kind = trailer_kind(fmt);
+  if (kind < 0) {
     fprintf(stderr, "zopfli-b200: unknown output format %d\n", (int)fmt);  // zopfli_lib.c:40 assert(0)
     abort();
   }
-  // gzip_container.c:84-124, zlib_container.c:50-79
-  const ChecksumKind kind = fmt == ZOPFLI_FORMAT_GZIP ? kCkCrc32 : kCkAdler32;
+  unsigned char bp = 0;
+  if (kind == kCkNone) {
+    body(&bp);
+    return;
+  }
   uint32_t sum = 0;
-  std::thread sum_thread([&] { sum = kind == kCkCrc32 ? crc32_parallel(in, insize) : adler32(in, insize); });  // overlaps the GPU work
+  std::thread sum_thread([&] { sum = host_checksum(in, insize, kind, 0); });  // overlaps the GPU work
   unsigned char hdr[10], tr[8];
   append_bytes(hdr, container_header(fmt, hdr), out, outsize);
   body(&bp);
@@ -302,6 +272,13 @@ void container_impl(const ZopfliOptions* options, ZopfliFormat fmt, const unsign
   if (debug_on()) fprintf(stderr, "[zb] api: %s join waited %.1f ms\n", kind == kCkCrc32 ? "crc" : "adler", now_ms() - tj);
   append_bytes(tr, container_trailer(kind, sum, insize, tr), out, outsize);
   if (options->verbose) report_size(fmt, insize, *outsize);
+}
+
+void compress_impl(const ZopfliOptions* options, ZopfliFormat fmt, const unsigned char* in, size_t insize,
+                   const unsigned char* dev_in, unsigned char** out, size_t* outsize) {
+  container_impl(options, fmt, in, insize, out, outsize, [&](unsigned char* bp) {
+    deflate_impl(options, 2, 1, in, insize, dev_in, bp, out, outsize);
+  });
 }
 
 void make_store(const unsigned short* ll, const unsigned short* dd, size_t n, Lz77Store& st) {
@@ -329,7 +306,7 @@ struct HostStaging : WaveStaging {
   }
   void stage(Engine& eng, int s, size_t len) override { eng.set_input_host(at(s, 0), len); }
   uint32_t checksum(Engine&, int s, size_t off, size_t n, int kind) override {
-    return kind == kCkCrc32 ? crc32_parallel(at(s, off), n) : adler32(at(s, off), n);
+    return host_checksum(at(s, off), n, kind, 0);
   }
   void read(Engine&, int s, size_t off, size_t n, unsigned char* dst) override { memcpy(dst, at(s, off), n); }
 };
@@ -381,8 +358,7 @@ struct ZopfliB200Compressor {
   double busy_ms = 0;                // time spent in Write and Finish
 
   ZopfliB200Compressor(const ZopfliOptions* o, ZopfliFormat f, WaveStaging* st)
-      : opt(*o), fmt(f), kind(f == ZOPFLI_FORMAT_GZIP ? kCkCrc32 : (f == ZOPFLI_FORMAT_ZLIB ? kCkAdler32 : kCkNone)),
-        staging(st), sum(kind == kCkAdler32 ? 1u : 0u) {
+      : opt(*o), fmt(f), kind(trailer_kind(f)), staging(st), sum(kind == kCkAdler32 ? 1u : 0u) {
     for (int s = WaveStaging::kSlots - 1; s >= 0; s--) free_slots.push_back(s);
   }
   ~ZopfliB200Compressor() {  // abandons unfinished work: waits for the waves in flight, drops their output
@@ -518,10 +494,7 @@ struct ZopfliB200Compressor {
     unsigned char tr[8];
     append_bytes(tr, container_trailer(kind, sum, received, tr), &pend, &pendsize);
     hand_out(out, outsize, true);
-    if (opt.verbose) {  // the reports ZopfliCompress prints after the deflate body and after the container
-      report_size(ZOPFLI_FORMAT_DEFLATE, received, (size_t)((deflate_bits + 7) / 8));
-      if (fmt != ZOPFLI_FORMAT_DEFLATE) report_size(fmt, received, produced);
-    }
+    if (opt.verbose) report_sizes(fmt, received, (size_t)((deflate_bits + 7) / 8), produced);
     layout.push_back(deflate_bits);
     busy_ms += now_ms() - t0;
     api_call_done(layout, now_ms() - busy_ms);
@@ -623,12 +596,12 @@ int ZopfliB200DeflateSpan(const ZopfliOptions* options, const unsigned char* in,
   return 0;
 }
 
-uint32_t ZopfliB200Crc32(const unsigned char* data, size_t size) { return crc32_parallel(data, size); }
+uint32_t ZopfliB200Crc32(const unsigned char* data, size_t size) { return host_checksum(data, size, kCkCrc32, 0); }
 uint32_t ZopfliB200Crc32Combine(uint32_t crc1, uint32_t crc2, uint64_t len2) { return crc32_combine(crc1, crc2, len2); }
 uint32_t ZopfliB200Adler32Combine(uint32_t adler1, uint32_t adler2, uint64_t len2) { return adler32_combine(adler1, adler2, len2); }
-uint32_t ZopfliB200Adler32(const unsigned char* data, size_t size) { return adler32(data, size); }
+uint32_t ZopfliB200Adler32(const unsigned char* data, size_t size) { return host_checksum(data, size, kCkAdler32, 0); }
 uint32_t ZopfliB200HostChecksumSliced(const unsigned char* data, size_t size, size_t slice_bytes, int kind) {
-  return checksum_sliced(data, size, slice_bytes, kind);
+  return host_checksum(data, size, kind, slice_bytes ? slice_bytes : 1);
 }
 
 int ZopfliB200AppendSpan(const unsigned char* span, size_t spansize, unsigned char* bp, unsigned char** out,
@@ -673,7 +646,7 @@ int ZopfliB200AppendSpan(const unsigned char* span, size_t spansize, unsigned ch
 int ZopfliB200CompressorNew(const ZopfliOptions* options, ZopfliFormat output_type, int device, void* cuda_stream,
                             ZopfliB200Compressor** c) {
   if (!options || !c) return 1;
-  if (output_type != ZOPFLI_FORMAT_GZIP && output_type != ZOPFLI_FORMAT_ZLIB && output_type != ZOPFLI_FORMAT_DEFLATE) return 1;
+  if (trailer_kind(output_type) < 0) return 1;
   WaveStaging* st = nullptr;
   if (device < 0) st = new HostStaging;
   else if (!g_device_staging || !(st = g_device_staging(device, cuda_stream))) return 1;

@@ -51,11 +51,14 @@ extern int (*g_pointer_device)(const void* p);
 // a compression call that started at t0 (now_ms) is done: `layout` becomes what
 // ZopfliB200LastMasterBitOffsets returns, and the call's time is added to ZopfliB200Stats::ms_total
 void api_call_done(std::vector<uint64_t>& layout, double t0);
+// the ChecksumKind of the trailer an output format carries (kCkNone for raw deflate), or -1 for a value
+// that is not a ZopfliFormat
+int trailer_kind(ZopfliFormat fmt);
 // header bytes of the gzip or zlib container (at most 10); 0 for raw deflate
 int container_header(ZopfliFormat fmt, unsigned char* hdr);
-// the verbose report after the deflate body (fmt DEFLATE, outsize = its bytes) or after the gzip / zlib
-// container (outsize = the whole output buffer), in the reference's formats
-void report_size(ZopfliFormat fmt, size_t insize, size_t outsize);
+// the verbose reports of a whole compression in the reference's formats: the deflate body's
+// (deflate_bytes), then with a gzip / zlib container the container's (outsize = the whole output)
+void report_sizes(ZopfliFormat fmt, size_t insize, size_t deflate_bytes, size_t outsize);
 // The pieces of ZopfliB200{Device,Host}EmitBlocks as the driver describes blocks (kFin symbols, input bytes
 // for stored pieces); plan and nbits are filled in by the caller.  False if bp0 > 7, a symbol is not a valid
 // literal / (length, distance), a range lies outside the store, or the store covers more than insize bytes.

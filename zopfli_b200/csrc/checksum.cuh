@@ -49,14 +49,8 @@ __device__ __forceinline__ uint32_t ck_load(const uint8_t* in, const CkLayout& L
   return la;
 }
 
-__device__ __forceinline__ uint32_t crc_slice8(uint32_t c, uint32_t lo, uint32_t hi, const uint32_t (*T)[256]) {
-  lo ^= c;
-  return T[7][lo & 255] ^ T[6][(lo >> 8) & 255] ^ T[5][(lo >> 16) & 255] ^ T[4][lo >> 24] ^ T[3][hi & 255] ^
-         T[2][(hi >> 8) & 255] ^ T[1][(hi >> 16) & 255] ^ T[0][hi >> 24];
-}
-
 __global__ void __launch_bounds__(kCkThreads) k_crc32(CkArgs a) {
-  __shared__ uint32_t T[8][256];  // slicing-by-8 tables (the host's crc32_range uses the same)
+  __shared__ uint32_t T[8][256];  // slicing-by-8 tables (the host checksum uses the same)
   for (uint32_t i = threadIdx.x; i < 256; i += kCkThreads) T[0][i] = crc_table_entry(0, i);
   __syncthreads();
   for (int t = 1; t < 8; t++) {

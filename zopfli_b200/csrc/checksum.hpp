@@ -1,6 +1,6 @@
 // CRC-32 (gzip trailer, gzip_container.c:27-81) and Adler-32 (zlib trailer, zlib_container.c:29-48) written
-// as sums of per-slice contributions that commute, shared by the sm_90a kernels (checksum.cuh), the host
-// checksums of api.cpp and the host seam ZopfliB200HostChecksumSliced.
+// as sums of per-slice contributions that commute, shared by the sm_90a kernels (checksum.cuh) and the host
+// checksum of api.cpp.
 //
 // CRC-32: crc0(s) is the CRC register after slice s starting from 0, without the final inversion.  crc0 is
 // linear over GF(2), so for an n-byte input cut into slices [a, b):
@@ -26,6 +26,14 @@ ZB_HD uint32_t crc_table_entry(int t, uint32_t i) {
   uint32_t c = i;
   for (int k = 0; k < 8 * (t + 1); k++) c = (c & 1) ? kCrcPoly ^ (c >> 1) : c >> 1;
   return c;
+}
+
+// slicing-by-8: the register c after the eight bytes lo (bytes 0-3, little-endian) and hi (bytes 4-7), with
+// T[t][i] = crc_table_entry(t, i)
+ZB_HD uint32_t crc_slice8(uint32_t c, uint32_t lo, uint32_t hi, const uint32_t (*T)[256]) {
+  lo ^= c;
+  return T[7][lo & 255] ^ T[6][(lo >> 8) & 255] ^ T[5][(lo >> 16) & 255] ^ T[4][lo >> 24] ^ T[3][hi & 255] ^
+         T[2][(hi >> 8) & 255] ^ T[1][(hi >> 16) & 255] ^ T[0][hi >> 24];
 }
 
 // a * b mod P in the reflected representation (32 fixed steps, no data-dependent exit)
@@ -110,33 +118,10 @@ ZB_HD int container_trailer(int kind, uint32_t checksum, uint64_t isize, uint8_t
   return 0;
 }
 
-// where the device kernels add their slices' contributions
+// slices' contributions added up: crc0 XORed, a and b summed (what crc_finish / adler_finish take)
 struct ChecksumAcc {
   uint32_t crc0, pad;
   unsigned long long a, b;
 };
-
-// The slice formulation on the host, one slice of `slice` bytes after the other, combined in reverse
-// order so that nothing depends on the order of the terms (the host seam ZopfliB200HostChecksumSliced).
-inline uint32_t checksum_sliced(const unsigned char* d, size_t n, size_t slice, int kind) {
-  if (slice == 0) slice = 1;
-  static const CrcShiftTable t = crc_shift_table();
-  uint32_t tab[256];
-  for (uint32_t i = 0; i < 256; i++) tab[i] = crc_table_entry(0, i);
-  ChecksumAcc acc = {0, 0, 0, 0};
-  for (size_t s = (n + slice - 1) / slice; s-- > 0;) {
-    const size_t a = s * slice, b = a + slice < n ? a + slice : n;
-    if (kind == kCkCrc32) {
-      uint32_t c = 0;
-      for (size_t i = a; i < b; i++) c = tab[(c ^ d[i]) & 255] ^ (c >> 8);
-      acc.crc0 ^= crc_shift(c, n - b, t);
-    } else {
-      const AdlerPart p = adler_chunk(d + a, b - a);
-      acc.a += p.s1;
-      acc.b += (p.s2 + ((n - b) % kAdlerMod) * p.s1) % kAdlerMod;
-    }
-  }
-  return kind == kCkCrc32 ? crc_finish(acc.crc0, n, t) : adler_finish(acc.a, acc.b, n);
-}
 
 }  // namespace zb

@@ -20,12 +20,11 @@ namespace {
 
 int compress_device_to_device(const ZopfliOptions* options, ZopfliFormat fmt, const unsigned char* dev_in,
                               size_t insize, void* stream, unsigned char** dev_out, size_t* outsize) {
-  if (!dev_out || !outsize || (fmt != ZOPFLI_FORMAT_GZIP && fmt != ZOPFLI_FORMAT_ZLIB && fmt != ZOPFLI_FORMAT_DEFLATE))
-    return 1;
+  const int ck = trailer_kind(fmt);
+  if (!dev_out || !outsize || ck < 0) return 1;
   const int dev = (insize == 0 && !dev_in) ? Engine::current_device() : Engine::pointer_device(dev_in);
   if (dev < 0) return 1;
   const double t0 = now_ms();
-  const int ck = fmt == ZOPFLI_FORMAT_GZIP ? kCkCrc32 : (fmt == ZOPFLI_FORMAT_ZLIB ? kCkAdler32 : kCkNone);
   Engine::Lease eng(dev);
   eng->set_input_device_copy(dev_in, insize, stream, ck);
   std::vector<Piece> pieces;
@@ -37,10 +36,7 @@ int compress_device_to_device(const ZopfliOptions* options, ZopfliFormat fmt, co
   const int hdr_len = container_header(fmt, hdr);
   size_t n = 0;
   unsigned char* out = eng->emit_to_device(ep, total, hdr, hdr_len, ck, stream, &n);
-  if (options->verbose) {  // the reports ZopfliCompress prints after the deflate body and after the container
-    report_size(ZOPFLI_FORMAT_DEFLATE, insize, (size_t)((total + 7) / 8));
-    if (fmt != ZOPFLI_FORMAT_DEFLATE) report_size(fmt, insize, n);
-  }
+  if (options->verbose) report_sizes(fmt, insize, (size_t)((total + 7) / 8), n);
   *dev_out = out;
   *outsize = n;
   api_call_done(layout, t0);

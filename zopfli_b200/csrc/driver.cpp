@@ -77,6 +77,8 @@ int usable_cpus() {
   return n < 1 ? 1 : n;
 }
 
+}  // namespace
+
 int host_threads() {
   static int n = [] {
     if (const char* e = getenv("ZOPFLI_B200_THREADS")) { int v = atoi(e); return v < 1 ? 1 : (v > 256 ? 256 : v); }
@@ -88,25 +90,7 @@ int host_threads() {
   return n;
 }
 
-template <typename F>
-void parallel_for(size_t n, F fn) {
-  int nt = (int)std::min<size_t>(n, (size_t)host_threads());
-  if (nt <= 1) {
-    for (size_t i = 0; i < n; i++) fn(i);
-    return;
-  }
-  std::atomic<size_t> next(0);
-  std::vector<std::thread> th;
-  for (int t = 0; t < nt; t++)
-    th.emplace_back([&] {
-      for (;;) {
-        size_t i = next.fetch_add(1);
-        if (i >= n) break;
-        fn(i);
-      }
-    });
-  for (auto& t : th) t.join();
-}
+namespace {
 
 // What the stages learn of one master block: A-B its cuts, C the size of every block's parse, D-E its pieces.
 struct Master {

@@ -3,6 +3,9 @@
 #include <stddef.h>
 #include <stdint.h>
 
+#include <algorithm>
+#include <atomic>
+#include <thread>
 #include <utility>
 #include <vector>
 
@@ -55,6 +58,31 @@ extern HostTimes g_host_times;
 double now_ms();
 // ZOPFLI_B200_DEBUG=1: timeline of the chunk pipelines and the API calls on stderr
 bool debug_on();
+
+// Host threads the library's CPU work may use: ZOPFLI_B200_THREADS, else the CPUs of the affinity mask and
+// the cgroup CPU quota (at most 32), shared among the LOCAL_WORLD_SIZE ranks of a box.
+int host_threads();
+
+// fn(0) ... fn(n - 1) on up to host_threads() threads, each taking the next index as it becomes free
+template <typename F>
+void parallel_for(size_t n, F fn) {
+  int nt = (int)std::min<size_t>(n, (size_t)host_threads());
+  if (nt <= 1) {
+    for (size_t i = 0; i < n; i++) fn(i);
+    return;
+  }
+  std::atomic<size_t> next(0);
+  std::vector<std::thread> th;
+  for (int t = 0; t < nt; t++)
+    th.emplace_back([&] {
+      for (;;) {
+        size_t i = next.fetch_add(1);
+        if (i >= n) break;
+        fn(i);
+      }
+    });
+  for (auto& t : th) t.join();
+}
 
 // Compresses the given byte ranges ("units": master blocks, or the single range of a
 // ZopfliDeflatePart call) of the input; the engine must already hold its bytes [in_base ...).
