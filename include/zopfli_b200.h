@@ -169,9 +169,10 @@ int ZopfliB200Adler32Device(const unsigned char* dev_in, size_t size, void* cuda
  * on its bytes, the 32 KiB before it and whether it is the last one, so the compressor runs the input as waves
  * of whole master blocks (half as many as ZopfliCompress runs at once on the device, so that the two waves in
  * flight fit the device memory of one call: about 72 on an 80 GB card by the driver's schedule; ZOPFLI_B200_BATCH and ZOPFLI_B200_CHUNKS shrink them) while more bytes arrive.
- *  - Identical bytes: every Write output followed by the Finish output, concatenated, equals
- *    ZopfliCompress(options, output_type, <all chunks concatenated>), for every chunking (zero-length writes
- *    included) and all three formats.  A compressor finished at once gives ZopfliCompress of an empty input.
+ *  - Identical bytes: without a flush or a dictionary (below), every Write output followed by the Finish
+ *    output, concatenated, equals ZopfliCompress(options, output_type, <all chunks concatenated>), for every
+ *    chunking (zero-length writes included) and all three formats.  A compressor finished at once gives
+ *    ZopfliCompress of an empty input.
  *  - Ownership: *out / *outsize follow ZopfliCompress's rule (bytes are appended under zopfli's capacity rule,
  *    the caller frees).  Only complete bytes are returned; the compressor keeps the partly filled last byte.
  *    The gzip / zlib header comes out with the first Write that returns bytes, or with Finish.
@@ -204,9 +205,48 @@ int ZopfliB200CompressorWrite(ZopfliB200Compressor* c, const unsigned char* chun
 int ZopfliB200CompressorFinish(ZopfliB200Compressor* c, unsigned char** out, size_t* outsize);
 /* Also valid before Finish: abandons the work (waits for the waves in flight, drops their output). */
 void ZopfliB200CompressorFree(ZopfliB200Compressor* c);
+/* Flush points and a preset dictionary, zlib's Z_SYNC_FLUSH / Z_FULL_FLUSH and deflateSetDictionary.
+ * Byte contract.  Let X = dictionary || data (the dictionary empty if none was set), positions in X, d = its
+ * length.  Flush calls cut the data into segments [s, e): the first starts at d, each Flush ends one and Finish
+ * ends the last.  The floor of a segment is the position of the most recent full flush at or before s, else 0.
+ * The deflate body is this chain of the reference's calls, each continuing at the bp and output buffer the one
+ * before left:
+ *  1. Data of a segment, if e > s or it is the last one: master blocks [s + i*1e6, min(s + (i+1)*1e6, e)), cut
+ *     as ZopfliDeflate cuts them (an empty last segment is one empty master block), each
+ *     ZopfliDeflatePart(options, 2, final, X + floor, mb_start - floor, mb_end - floor, ...) over X[floor, e);
+ *     final is 1 only on the last master block of the last segment.
+ *  2. End of a flushed segment: ZopfliDeflatePart(options, 0, 0, X, e, e, ...), the sync marker (a stored block
+ *     of BFINAL 0 and LEN 0, deflate.c:625-663).  Every Flush call emits exactly one marker; a flushed segment
+ *     with no bytes contributes only the marker.
+ * So only the last 32 KiB of the dictionary can influence the output, and after a full flush neither the
+ * dictionary nor earlier data can.  With no dictionary and no flush this is ZopfliDeflate of the data: the
+ * identical-bytes rule above.  Containers: gzip as always, and a dictionary is refused (the format has no field
+ * for one; zlib refuses it the same way).  zlib without a dictionary as always (78 DA); with one, 78 F9 (FDICT)
+ * and DICTID, the big-endian Adler-32 of the whole dictionary, as deflateSetDictionary writes it (1 for 0 bytes).
+ * In every format the trailer's checksum and ISIZE cover the data only.
+ * Flush compresses everything written so far as one wave, however short (later waves count master blocks from
+ * the flush point), waits for every wave in flight and appends all remaining output: the header if it has not
+ * gone out, the segment's blocks and the marker.  The stream is then byte-aligned: nothing stays behind.  It
+ * returns nonzero, every output untouched, for a NULL c, out or outsize, a mode other than 2 or 3, and after
+ * Finish.  The staging bound stays 3 x (wave bytes + 32 KiB + 16).
+ * SetDictionary is accepted once, before the first Write or Flush call of any length.  dict is memory of the
+ * kind the compressor takes for chunks: host memory for a host compressor, or that device's memory for a device
+ * compressor, ordered after cuda_stream; the DICTID of a device dictionary is computed on the device
+ * (k_adler32), so the dictionary does not cross PCIe.  Its last 32 KiB are staged in front of the first wave.
+ * It returns nonzero, nothing changed, for gzip, a NULL c, a NULL dict with n > 0, the wrong kind of memory, a
+ * second call, and a call after the first Write or Flush.
+ * Reports: after Finish, ZopfliB200LastMasterBitOffsets gives the bit offset of every master block of every
+ * segment in stream order (the bit positions before each data call above), then the end offset.  With
+ * verbose, each flush wave prints its reports as a wave does. */
+#define ZOPFLI_B200_SYNC_FLUSH 2 /* zlib's Z_SYNC_FLUSH */
+#define ZOPFLI_B200_FULL_FLUSH 3 /* zlib's Z_FULL_FLUSH */
+int ZopfliB200CompressorFlush(ZopfliB200Compressor* c, int mode, unsigned char** out, size_t* outsize);
+int ZopfliB200CompressorSetDictionary(ZopfliB200Compressor* c, const unsigned char* dict, size_t n);
 /* The compressor's wave policy as a pure function (csrc/dist_layout.hpp next_wave; no GPU needed): with
- * `received` bytes written, Finish called or not, `handed` bytes already in waves and waves of wave_blocks
- * master blocks, returns 1 and the next wave [*a, *b) with its BFINAL flag, or 0 when no wave is ready. */
+ * `received` bytes written, `handed` bytes already in waves and waves of wave_blocks master blocks, returns 1 and
+ * the next wave [*a, *b) with its BFINAL flag, or 0 when no wave is ready.  finished: 0 while writing (a wave is
+ * whole master blocks from `handed` with a byte past it), 1 at Finish (all that is left, final), 2 at a flush
+ * (all that is left, not final; 0 when handed == received). */
 int ZopfliB200CompressorWave(size_t received, int finished, size_t handed, size_t wave_blocks, size_t* a, size_t* b,
                              int* final);
 

@@ -7,7 +7,11 @@ rate, and the device memory in use after it (cudaMemGetInfo), so that growth acr
 compressor output is checked against ZopfliCompress's.  The card's name, power limit and clock limit are read
 in the same run.
 
-    python tools/compressor_bench.py [--mib 430] [--reps 3] [--numiterations 15]
+With --flush-every BYTES, two more legs (host and device chunks, 64 MiB writes) end a sync flush every BYTES of
+input: each flush runs what has arrived as a wave of its own, however short.  Their output differs from
+ZopfliCompress's by the flush points, so it is checked by inflating it instead.
+
+    python tools/compressor_bench.py [--mib 430] [--reps 3] [--numiterations 15] [--flush-every BYTES]
 """
 import argparse
 import json
@@ -15,6 +19,7 @@ import os
 import subprocess
 import sys
 import time
+import zlib
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
@@ -39,11 +44,18 @@ def run_whole(lib, data, kw):
     return lib.compress_ptr(a.ctypes.data, len(data), zb.ZOPFLI_FORMAT_GZIP, **kw)
 
 
-def run_pieces(lib, src, write, kw, device):
+def run_pieces(lib, src, write, kw, device, flush_every=0):
     out = []
     with lib.compressobj(zb.ZOPFLI_FORMAT_GZIP, device=0 if device else None, **kw) as c:
-        for p in range(0, len(src), write):
-            out.append(c.compress(src[p:p + write]))
+        p = 0
+        while p < len(src):
+            q = min(p + write, len(src))
+            if flush_every:
+                q = min(q, (p // flush_every + 1) * flush_every)
+            out.append(c.compress(src[p:q]))
+            p = q
+            if flush_every and p % flush_every == 0:
+                out.append(c.flush(zlib.Z_SYNC_FLUSH))
         out.append(c.flush())
     return b"".join(out)
 
@@ -53,6 +65,7 @@ def main():
     ap.add_argument("--mib", type=int, default=430)
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--numiterations", type=int, default=15)
+    ap.add_argument("--flush-every", type=int, default=0, help="bytes of input between sync flushes (0: no flush legs)")
     args = ap.parse_args()
     kw = {"numiterations": args.numiterations}
     lib = zb.library()
@@ -67,6 +80,12 @@ def main():
         legs.append(("compressor host %d MiB" % write, lambda w=write: run_pieces(lib, host_view, w * MIB, kw, False)))
     for write in (1, 64):
         legs.append(("compressor device %d MiB" % write, lambda w=write: run_pieces(lib, dev, w * MIB, kw, True)))
+    f = args.flush_every
+    if f:
+        legs.append(("compressor host 64 MiB, sync flush every %d B" % f,
+                     lambda: run_pieces(lib, host_view, 64 * MIB, kw, False, f)))
+        legs.append(("compressor device 64 MiB, sync flush every %d B" % f,
+                     lambda: run_pieces(lib, dev, 64 * MIB, kw, True, f)))
     want = None
     for rep in range(args.reps):
         for name, fn in legs:
@@ -78,9 +97,14 @@ def main():
             if want is None:
                 want = got
             free, total = torch.cuda.mem_get_info(0)
-            print(json.dumps({"rep": rep, "leg": name, "ms": round(ms, 1), "MiB_s": round(len(data) / MIB / (ms / 1e3), 2),
-                              "out_bytes": len(got), "identical": got == want,
-                              "device_used_GiB": round((total - free) / (1 << 30), 2)}), flush=True)
+            rec = {"rep": rep, "leg": name, "ms": round(ms, 1), "MiB_s": round(len(data) / MIB / (ms / 1e3), 2),
+                   "out_bytes": len(got)}
+            if "flush" in name:
+                rec["inflates"] = zlib.decompress(got, 31) == data
+            else:
+                rec["identical"] = got == want
+            rec["device_used_GiB"] = round((total - free) / (1 << 30), 2)
+            print(json.dumps(rec), flush=True)
     print(json.dumps({"card": card()}), flush=True)
 
 

@@ -10,6 +10,7 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+import zlib
 
 import numpy as np
 
@@ -57,7 +58,8 @@ EXPORTS = ["ZopfliInitOptions", "ZopfliCompress", "ZopfliDeflate", "ZopfliDeflat
            "ZopfliB200GetStats", "ZopfliB200ResetStats", "ZopfliB200SetStream", "ZopfliB200Device",
            "ZopfliB200Version", "ZopfliB200CompressDeviceToDevice", "ZopfliB200FreeDevice", "ZopfliB200Crc32Device",
            "ZopfliB200Adler32Device", "ZopfliB200HostChecksumSliced", "ZopfliB200CompressorNew", "ZopfliB200CompressorWrite",
-           "ZopfliB200CompressorFinish", "ZopfliB200CompressorFree", "ZopfliB200CompressorWave"]
+           "ZopfliB200CompressorFinish", "ZopfliB200CompressorFree", "ZopfliB200CompressorWave",
+           "ZopfliB200CompressorFlush", "ZopfliB200CompressorSetDictionary"]
 
 
 def _pad(data):
@@ -208,6 +210,10 @@ class Library:
         L.ZopfliB200CompressorWrite.restype = C.c_int
         L.ZopfliB200CompressorFinish.argtypes = [vp, C.POINTER(vp), C.POINTER(sz)]
         L.ZopfliB200CompressorFinish.restype = C.c_int
+        L.ZopfliB200CompressorFlush.argtypes = [vp, C.c_int, C.POINTER(vp), C.POINTER(sz)]
+        L.ZopfliB200CompressorFlush.restype = C.c_int
+        L.ZopfliB200CompressorSetDictionary.argtypes = [vp, vp, sz]
+        L.ZopfliB200CompressorSetDictionary.restype = C.c_int
         L.ZopfliB200CompressorFree.argtypes = [vp]
         L.ZopfliB200CompressorFree.restype = None
         L.ZopfliB200CompressorWave.argtypes = [sz, C.c_int, sz, sz, C.POINTER(sz), C.POINTER(sz), C.POINTER(C.c_int)]
@@ -523,18 +529,21 @@ class Library:
         return self._device_checksum(self.lib.ZopfliB200Adler32Device, t, stream)
 
     # ---- input in pieces (ZopfliB200Compressor) ----
-    def compressobj(self, fmt=ZOPFLI_FORMAT_GZIP, device=None, stream=None, **kw) -> "Compressor":
-        """A compressor shaped like zlib.compressobj: compress(chunk) -> bytes, flush() -> bytes.  All outputs
-        concatenated equal compress(<all chunks>, fmt, **kw).  device=None: chunks are bytes-like objects;
-        device=<index or torch.device>: chunks are contiguous CUDA tensors of that device, each copied after
-        the work queued on `stream`, or, without stream=, on the tensor's current stream (a private stream of the
-        compressor waits for it, so the caller's streams gain no dependency)."""
-        return Compressor(self, fmt, device, stream, **kw)
+    def compressobj(self, fmt=ZOPFLI_FORMAT_GZIP, device=None, stream=None, zdict=None, **kw) -> "Compressor":
+        """A compressor shaped like zlib.compressobj: compress(chunk) -> bytes, flush(mode) -> bytes.  Without
+        zdict and sync / full flushes, all outputs concatenated equal compress(<all chunks>, fmt, **kw).
+        device=None: chunks are bytes-like objects; device=<index or torch.device>: chunks are contiguous CUDA
+        tensors of that device, each copied after the work queued on `stream`, or, without stream=, on the
+        tensor's current stream (a private stream of the compressor waits for it, so the caller's streams gain
+        no dependency).  zdict: a preset dictionary (zlib and raw deflate only), bytes-like, or for a device
+        compressor also a contiguous uint8 CUDA tensor of its device."""
+        return Compressor(self, fmt, device, stream, zdict, **kw)
 
     def compressor_wave(self, received, finished, handed, wave_blocks):
-        """the compressor's next wave (a, b, final), or None (ZopfliB200CompressorWave)"""
+        """the compressor's next wave (a, b, final), or None (ZopfliB200CompressorWave); finished: 0 or False while
+        writing, 1 or True at Finish, 2 at a flush"""
         a, b, f = C.c_size_t(0), C.c_size_t(0), C.c_int(0)
-        if not self.lib.ZopfliB200CompressorWave(received, 1 if finished else 0, handed, wave_blocks, C.byref(a), C.byref(b),
+        if not self.lib.ZopfliB200CompressorWave(received, int(finished), handed, wave_blocks, C.byref(a), C.byref(b),
                                                  C.byref(f)):
             return None
         return a.value, b.value, bool(f.value)
@@ -619,8 +628,10 @@ class Compressor:
     """ZopfliB200Compressor: input in pieces, ZopfliCompress's bytes out (include/zopfli_b200.h, "input in
     pieces").  Use it as a context manager, or close() it; closing an unfinished compressor abandons it."""
 
-    def __init__(self, lib, fmt=ZOPFLI_FORMAT_GZIP, device=None, stream=None, **kw):
+    def __init__(self, lib, fmt=ZOPFLI_FORMAT_GZIP, device=None, stream=None, zdict=None, **kw):
         self._c = None
+        if zdict is not None and fmt == ZOPFLI_FORMAT_GZIP:
+            raise ValueError("gzip has no field for a preset dictionary")
         self._lib, self._stream = lib, None
         dev = -1
         if device is not None:
@@ -642,6 +653,39 @@ class Compressor:
                                            C.byref(handle)) != 0:
             raise ValueError("ZopfliB200CompressorNew: unknown format, or no such device")
         self._c = handle
+        if zdict is not None:
+            try:
+                self._set_dictionary(zdict)
+            except BaseException:
+                self.close()
+                raise
+
+    def _set_dictionary(self, zdict):
+        if self._dev >= 0:
+            import torch
+            if not isinstance(zdict, torch.Tensor):  # bytes-like: copied to the device on the compressor's stream
+                host = np.frombuffer(memoryview(zdict).cast("B"), np.uint8)
+                with torch.cuda.stream(self._stream):
+                    zdict = torch.from_numpy(host.copy()).to(torch.device("cuda", self._dev))
+            elif zdict.dtype != torch.uint8:
+                raise ValueError("a device dictionary is a uint8 tensor")
+            ptr, nbytes = self._chunk(zdict)
+            rc = self._lib.lib.ZopfliB200CompressorSetDictionary(self._c, C.c_void_p(ptr), nbytes)
+        else:
+            a = np.frombuffer(memoryview(zdict).cast("B"), np.uint8)
+            rc = self._lib.lib.ZopfliB200CompressorSetDictionary(self._c, a.ctypes.data if len(a) else None, len(a))
+        if rc != 0:
+            raise ValueError("ZopfliB200CompressorSetDictionary refused the dictionary (wrong kind of memory)")
+
+    def _chunk(self, t):
+        """(address, nbytes) of a device chunk, with the compressor's stream ordered after t's current stream"""
+        import torch
+        if not isinstance(t, torch.Tensor):
+            raise ValueError("a device compressor takes CUDA tensors")
+        ptr, nbytes = _device_bytes(t)
+        if not self._own_stream:  # ordered after the chunk's current stream, as compress_device is
+            self._stream.wait_stream(torch.cuda.current_stream(t.device))
+        return ptr, nbytes
 
     def _call(self, fn, *args):
         if self._c is None:
@@ -654,19 +698,23 @@ class Compressor:
     def compress(self, chunk) -> bytes:
         """the output bytes that are complete after this chunk (possibly none)"""
         if self._dev >= 0:
-            import torch
-            if not isinstance(chunk, torch.Tensor):
-                raise ValueError("a device compressor takes CUDA tensors")
-            ptr, nbytes = _device_bytes(chunk)
-            if not self._own_stream:  # ordered after the chunk's current stream, as compress_device is
-                self._stream.wait_stream(torch.cuda.current_stream(chunk.device))
+            ptr, nbytes = self._chunk(chunk)
             return self._call(self._lib.lib.ZopfliB200CompressorWrite, C.c_void_p(ptr), nbytes)
         a = np.frombuffer(memoryview(chunk).cast("B"), np.uint8)
         return self._call(self._lib.lib.ZopfliB200CompressorWrite, a.ctypes.data if len(a) else None, len(a))
 
-    def flush(self) -> bytes:
-        """the rest of the stream with the trailer; the compressor takes no more input"""
-        return self._call(self._lib.lib.ZopfliB200CompressorFinish)
+    def flush(self, mode=zlib.Z_FINISH) -> bytes:
+        """zlib's flush modes.  Z_FINISH (the default): the rest of the stream with the trailer; the compressor
+        takes no more input.  Z_SYNC_FLUSH: everything written so far, byte-aligned and decodable, ending with an
+        empty stored block.  Z_FULL_FLUSH: the same, and no later byte refers to what came before, so inflating
+        can start there.  Z_NO_FLUSH: nothing."""
+        if mode == zlib.Z_FINISH:
+            return self._call(self._lib.lib.ZopfliB200CompressorFinish)
+        if mode in (zlib.Z_SYNC_FLUSH, zlib.Z_FULL_FLUSH):
+            return self._call(self._lib.lib.ZopfliB200CompressorFlush, mode)
+        if mode == zlib.Z_NO_FLUSH:
+            return b""
+        raise ValueError("unsupported flush mode %r: Z_NO_FLUSH, Z_SYNC_FLUSH, Z_FULL_FLUSH or Z_FINISH" % (mode,))
 
     def close(self):
         if self._c is not None:
@@ -697,6 +745,6 @@ def compress(data: bytes, fmt: int = ZOPFLI_FORMAT_GZIP, **options) -> bytes:
     return library().compress(data, fmt, **options)
 
 
-def compressobj(fmt: int = ZOPFLI_FORMAT_GZIP, device=None, stream=None, **options) -> Compressor:
+def compressobj(fmt: int = ZOPFLI_FORMAT_GZIP, device=None, stream=None, zdict=None, **options) -> Compressor:
     """a compressor fed in pieces (Library.compressobj), like zlib.compressobj"""
-    return library().compressobj(fmt, device, stream, **options)
+    return library().compressobj(fmt, device, stream, zdict, **options)

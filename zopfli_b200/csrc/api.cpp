@@ -49,18 +49,20 @@ int trailer_kind(ZopfliFormat fmt) {
 }
 
 // header bytes of the gzip (gzip_container.c:95-104) or zlib (zlib_container.c:58-64) container; 0 for raw deflate
-int container_header(ZopfliFormat fmt, unsigned char* hdr) {
+int container_header(ZopfliFormat fmt, unsigned char* hdr, const uint32_t* dictid) {
   if (fmt == ZOPFLI_FORMAT_GZIP) {
     static const unsigned char gz[10] = {31, 139, 8, 0, 0, 0, 0, 0, 2, 3};
     memcpy(hdr, gz, 10);
     return 10;
   }
   if (fmt == ZOPFLI_FORMAT_ZLIB) {
-    unsigned cmfflg = 256 * 120 + 3 * 64;
+    unsigned cmfflg = 256 * 120 + 3 * 64 + (dictid ? 32 : 0);  // FDICT: 78 F9, as zlib's deflateSetDictionary
     cmfflg += 31 - cmfflg % 31;
     hdr[0] = (unsigned char)(cmfflg / 256);
     hdr[1] = (unsigned char)(cmfflg % 256);
-    return 2;
+    if (!dictid) return 2;
+    for (int i = 0; i < 4; i++) hdr[2 + i] = (unsigned char)(*dictid >> (24 - 8 * i));
+    return 6;
   }
   return 0;
 }
@@ -309,6 +311,7 @@ struct HostStaging : WaveStaging {
     return host_checksum(at(s, off), n, kind, 0);
   }
   void read(Engine&, int s, size_t off, size_t n, unsigned char* dst) override { memcpy(dst, at(s, off), n); }
+  uint32_t checksum_of(const unsigned char* p, size_t n, int kind) override { return host_checksum(p, n, kind, 0); }
 };
 
 }  // namespace
@@ -324,10 +327,13 @@ int (*g_pointer_device)(const void*) = nullptr;
 // into span records plus the checksum of its bytes.  The next wave's slot takes over the last 32 KiB as its
 // dictionary.  Waves are spliced onto the stream in order, at its bit phase, by the calling thread; only the
 // complete bytes go back to the caller.
+// Positions are counted in X = preset dictionary || data.  A flush ends a segment: what is left becomes one
+// wave however short, the sync marker follows it, and the next segment's master blocks count from there.  A
+// full flush also raises the floor, the first position a later parse may see: the next slot starts there.
 struct ZopfliB200Compressor {
   struct Run {
     Wave w;
-    size_t base;        // stream position of the slot's byte 0
+    size_t base;        // position of the slot's byte 0
     int slot;
     SpanRecords sr;
     uint32_t sum = 0;   // checksum of the wave's bytes [w.a, w.b)
@@ -340,10 +346,15 @@ struct ZopfliB200Compressor {
   int kind;
   std::unique_ptr<WaveStaging> staging;
   size_t wave_blocks = 0;            // master blocks per wave, set when the first byte arrives
-  size_t received = 0, handed = 0;   // bytes written; bytes that belong to waves
+  size_t received = 0, handed = 0;   // positions: end of the bytes written; end of the bytes in waves
+  size_t dict_len = 0;               // position of the first data byte
+  size_t floor = 0;                  // position of the last full flush
+  bool started = false;              // a Write or Flush was accepted: no dictionary any more
+  bool has_dict = false;
+  uint32_t dictid = 0;               // Adler-32 of the whole dictionary
   bool finished = false;
   int fill = -1;                     // slot taking the next bytes (-1: none yet)
-  size_t fill_base = 0;              // stream position of its byte 0
+  size_t fill_base = 0;              // position of its byte 0
   std::vector<int> free_slots;
   std::deque<std::unique_ptr<Run>> inflight;
   // the stream not yet returned: at most the partly filled last byte between calls (zopfli-style buffer)
@@ -379,7 +390,7 @@ struct ZopfliB200Compressor {
   // the caller's bytes up to stream position `upto` into the filling slot; chunk starts at position `at`
   void fill_to(size_t upto, const unsigned char* chunk, size_t at) {
     if (upto == received) return;
-    if (fill < 0) take_slot(0);
+    if (fill < 0) take_slot(floor);
     staging->put(fill, received - fill_base, chunk + (received - at), upto - received);
     received = upto;
   }
@@ -407,10 +418,11 @@ struct ZopfliB200Compressor {
     r.done = true;
   }
 
-  // starts wave w on the filling slot; a wave that is not the last hands its last 32 KiB to a fresh slot
+  // starts wave w on the filling slot; a wave that is not the last hands its last 32 KiB above the floor to a
+  // fresh slot
   void launch(const Wave& w) {
     while (inflight.size() >= max_inflight()) retire_oldest();
-    if (fill < 0) take_slot(0);  // an empty stream
+    if (fill < 0) take_slot(floor);  // an empty stream
     std::unique_ptr<Run> r(new Run);
     r->w = w;
     r->base = fill_base;
@@ -421,9 +433,16 @@ struct ZopfliB200Compressor {
     handed = w.b;
     fill = -1;
     if (w.final) return;
-    const size_t base = wave_base(w.b);
+    const size_t base = wave_base(w.b, floor);
     take_slot(base);
     staging->carry(p->slot, base - p->base, fill, w.b - base);
+  }
+
+  void put_header() {
+    if (header_done) return;
+    unsigned char hdr[10];
+    append_bytes(hdr, container_header(fmt, hdr, has_dict ? &dictid : nullptr), &pend, &pendsize);
+    header_done = true;
   }
 
   // the oldest wave in flight, once done, spliced onto the stream (with the block reports of verbose)
@@ -431,11 +450,7 @@ struct ZopfliB200Compressor {
     std::unique_ptr<Run> r = std::move(inflight.front());
     inflight.pop_front();
     r->worker.join();
-    if (!header_done) {
-      unsigned char hdr[10];
-      append_bytes(hdr, container_header(fmt, hdr), &pend, &pendsize);
-      header_done = true;
-    }
+    put_header();
     const unsigned phase = pendsize ? (bp & 7u) : 0u;
     std::vector<Engine::EmitPiece> ep;
     std::vector<uint64_t> ub;
@@ -464,9 +479,25 @@ struct ZopfliB200Compressor {
     if (keep) append_bytes(&last, 1, &pend, &pendsize);
   }
 
+  int set_dictionary(const unsigned char* dict, size_t n) {
+    if (fmt == ZOPFLI_FORMAT_GZIP || started || has_dict || (!dict && n) || !staging->accepts(dict, n)) return 1;
+    const double t0 = now_ms();
+    has_dict = true;
+    dictid = n ? staging->checksum_of(dict, n, kCkAdler32) : 1u;
+    if (n) {  // only the last 32 KiB can be matched: they go in front of the first wave
+      set_wave_blocks();
+      take_slot(wave_base(n));
+      staging->put(fill, 0, dict + fill_base, n - fill_base);
+    }
+    received = handed = dict_len = n;
+    busy_ms += now_ms() - t0;
+    return 0;
+  }
+
   int write(const unsigned char* chunk, size_t n, unsigned char** out, size_t* outsize) {
     if (!out || !outsize || finished || !staging->accepts(chunk, n)) return 1;
     const double t0 = now_ms();
+    started = true;
     if (n) {
       set_wave_blocks();
       const size_t at = received, total = received + n;
@@ -483,18 +514,47 @@ struct ZopfliB200Compressor {
     return 0;
   }
 
+  // mode 2 (sync) or 3 (full): what is left becomes one wave, then the marker, a stored block of BFINAL 0 and
+  // LEN 0 (ZopfliDeflatePart with btype 0 over an empty range, deflate.c:625-663); the stream is byte-aligned
+  int flush(int mode, unsigned char** out, size_t* outsize) {
+    if (!out || !outsize || finished || (mode != 2 && mode != 3)) return 1;
+    const double t0 = now_ms();
+    started = true;
+    Wave w;
+    const bool full = mode == 3;
+    if (next_wave(received, kWaveFlush, handed, wave_blocks, &w)) {
+      if (full) floor = w.b;  // before launch: the next slot starts at the floor, with nothing carried
+      launch(w);
+    } else if (full) {
+      floor = received;
+      if (fill >= 0) fill_base = floor;  // the filling slot holds nothing past the floor: drop what it carried
+    }
+    while (!inflight.empty()) retire_oldest();
+    put_header();
+    SpanPiece marker;
+    marker.stored = true;
+    marker.final = false;
+    marker.instart = marker.inend = 0;
+    splice_pieces({marker}, nullptr, &bp, &pend, &pendsize);
+    deflate_bits = stored_end(deflate_bits, 0);
+    hand_out(out, outsize, true);
+    busy_ms += now_ms() - t0;
+    return 0;
+  }
+
   int finish(unsigned char** out, size_t* outsize) {
     if (!out || !outsize || finished) return 1;
     const double t0 = now_ms();
     finished = true;
     Wave w;
-    next_wave(received, true, handed, wave_blocks, &w);
+    next_wave(received, kWaveFinish, handed, wave_blocks, &w);
     launch(w);
     while (!inflight.empty()) retire_oldest();
+    const size_t insize = received - dict_len;
     unsigned char tr[8];
-    append_bytes(tr, container_trailer(kind, sum, received, tr), &pend, &pendsize);
+    append_bytes(tr, container_trailer(kind, sum, insize, tr), &pend, &pendsize);
     hand_out(out, outsize, true);
-    if (opt.verbose) report_sizes(fmt, received, (size_t)((deflate_bits + 7) / 8), produced);
+    if (opt.verbose) report_sizes(fmt, insize, (size_t)((deflate_bits + 7) / 8), produced);
     layout.push_back(deflate_bits);
     busy_ms += now_ms() - t0;
     api_call_done(layout, now_ms() - busy_ms);
@@ -663,12 +723,21 @@ int ZopfliB200CompressorFinish(ZopfliB200Compressor* c, unsigned char** out, siz
   return c ? c->finish(out, outsize) : 1;
 }
 
+int ZopfliB200CompressorFlush(ZopfliB200Compressor* c, int mode, unsigned char** out, size_t* outsize) {
+  return c ? c->flush(mode, out, outsize) : 1;
+}
+
+int ZopfliB200CompressorSetDictionary(ZopfliB200Compressor* c, const unsigned char* dict, size_t n) {
+  return c ? c->set_dictionary(dict, n) : 1;
+}
+
 void ZopfliB200CompressorFree(ZopfliB200Compressor* c) { delete c; }
 
 int ZopfliB200CompressorWave(size_t received, int finished, size_t handed, size_t wave_blocks, size_t* a, size_t* b,
                              int* final) {
   Wave w;
-  if (!next_wave(received, finished != 0, handed, wave_blocks, &w)) return 0;
+  const int call = finished == kWaveFlush ? (int)kWaveFlush : (finished != 0 ? (int)kWaveFinish : (int)kWaveWrite);
+  if (!next_wave(received, call, handed, wave_blocks, &w)) return 0;
   *a = w.a;
   *b = w.b;
   *final = w.final ? 1 : 0;

@@ -41,6 +41,8 @@ struct WaveStaging {
   virtual uint32_t checksum(Engine& eng, int s, size_t off, size_t n, int kind) = 0;
   // slot s's bytes [off, off + n) to dst
   virtual void read(Engine& eng, int s, size_t off, size_t n, unsigned char* dst) = 0;
+  // CRC-32 / Adler-32 of n bytes at p, memory of the kind this staging takes (a preset dictionary)
+  virtual uint32_t checksum_of(const unsigned char* p, size_t n, int kind) = 0;
 };
 // The device side of ZopfliB200CompressorNew, registered by device_api.cpp (null in a host-only build): a
 // staging on device dev, ordered after cuda_stream, or null when dev is not a usable device.
@@ -54,8 +56,9 @@ void api_call_done(std::vector<uint64_t>& layout, double t0);
 // the ChecksumKind of the trailer an output format carries (kCkNone for raw deflate), or -1 for a value
 // that is not a ZopfliFormat
 int trailer_kind(ZopfliFormat fmt);
-// header bytes of the gzip or zlib container (at most 10); 0 for raw deflate
-int container_header(ZopfliFormat fmt, unsigned char* hdr);
+// header bytes of the gzip or zlib container (at most 10); 0 for raw deflate.  With dictid, the zlib header
+// of a stream with a preset dictionary: FDICT set and the dictionary's Adler-32 (RFC 1950, 2.2).
+int container_header(ZopfliFormat fmt, unsigned char* hdr, const uint32_t* dictid = nullptr);
 // the verbose reports of a whole compression in the reference's formats: the deflate body's
 // (deflate_bytes), then with a gzip / zlib container the container's (outsize = the whole output)
 void report_sizes(ZopfliFormat fmt, size_t insize, size_t deflate_bytes, size_t outsize);

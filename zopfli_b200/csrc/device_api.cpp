@@ -102,6 +102,10 @@ struct DeviceWaveStaging : WaveStaging {
     return eng.checksum_device(slot[s] + off, n, ds.stream(), kind);
   }
   void read(Engine& eng, int s, size_t off, size_t n, unsigned char* dst) override { eng.download(slot[s] + off, dst, n); }
+  uint32_t checksum_of(const unsigned char* p, size_t n, int kind) override {  // k_crc32 / k_adler32: no PCIe copy
+    Engine::Lease eng(ds.device());
+    return eng->checksum_device(p, n, user_stream, kind);
+  }
 };
 
 WaveStaging* device_staging(int dev, void* stream) {

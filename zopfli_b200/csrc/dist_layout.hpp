@@ -29,12 +29,19 @@ inline std::vector<std::pair<size_t, size_t>> master_blocks(size_t a, size_t b) 
 
 // The next wave of a compressor fed in pieces (ZopfliB200Compressor): `received` bytes have arrived,
 // `handed` of them already belong to waves, and a wave is `wave_blocks` master blocks.  A wave is whole
-// master blocks counted from byte 0 of the stream.  Before Finish a wave is released only once a byte past
-// it has arrived, because its last master block's BFINAL depends on whether more input follows; at Finish
-// everything left is one final wave (an empty stream: one empty final wave).  Returns false when no wave
-// is ready.  After a final wave there is none.
+// master blocks counted from the start of its segment (the stream's first byte, or the last flush point).
+// Before Finish a wave is released only once a byte past it has arrived, because its last master block's
+// BFINAL depends on whether more input follows; at Finish (finished == 1) everything left is one final wave
+// (an empty stream or segment: one empty final wave).  At a flush (finished == 2) everything left is one
+// wave that is not final, or none when nothing is left.  Returns false when no wave is ready.  After a final
+// wave there is none.
 struct Wave { size_t a, b; bool final; };
-inline bool next_wave(size_t received, bool finished, size_t handed, size_t wave_blocks, Wave* w) {
+enum WaveCall { kWaveWrite = 0, kWaveFinish = 1, kWaveFlush = 2 };
+inline bool next_wave(size_t received, int finished, size_t handed, size_t wave_blocks, Wave* w) {
+  if (finished == kWaveFlush) {
+    *w = {handed, received, false};
+    return received > handed;
+  }
   if (finished) {
     *w = {handed, received, true};
     return true;
@@ -46,8 +53,12 @@ inline bool next_wave(size_t received, bool finished, size_t handed, size_t wave
 }
 
 // Where a wave's staged bytes start: the 32 KiB dictionary in front of byte a (squeeze.c:229-230), rounded
-// down to 16 bytes for the kernels' vector loads, as ZopfliB200DeflateSpan and dist_shard stage it.
-inline size_t wave_base(size_t a) { return a > (size_t)kWindow ? (a - kWindow) & ~(size_t)15 : 0; }
+// down to 16 bytes for the kernels' vector loads, as ZopfliB200DeflateSpan and dist_shard stage it.  With a
+// floor (a compressor's last full flush) no byte before it is staged: the parse then sees none of them.
+inline size_t wave_base(size_t a, size_t floor = 0) {
+  const size_t b = a > (size_t)kWindow ? (a - kWindow) & ~(size_t)15 : 0;
+  return b > floor ? b : floor;
+}
 
 // Rank `rank` of `world` owns the master blocks [rank*nm/world, (rank+1)*nm/world): bytes [a, b).  Its
 // device copy starts at `base` <= a: the 32 KiB dictionary in front of the shard (squeeze.c:229-230),
