@@ -10,6 +10,7 @@ import os
 import numpy as np
 import pytest
 
+import run_list_fixtures
 import zref
 from zopfli_b200 import corpus
 
@@ -29,6 +30,9 @@ CASES = [
     ("tiny1", b"a", 0, 1),
     ("tail-repeat", b"xyz" * 200 + b"aaaa", 100, 604),
 ]
+# run lists of more than eight runs (run_list_fixtures.py), each range from 11000 bytes before its first full R, so
+# that the match-table seam's first 12000 positions include it
+CASES += [("runs-" + c, d, max(s, run_list_fixtures.r_at(c) - 11000), e) for c, d, s, e in run_list_fixtures.all_cases()]
 
 
 @pytest.mark.parametrize("name,data,s,e", CASES, ids=[c[0] for c in CASES])
@@ -130,6 +134,8 @@ INT_DP_CASES = [
     ("longrun-cut", corpus.adv_longrun(), 1000, 68000, 3),
     ("random", corpus.random_bytes(200000), 0, 200000, 3),
 ]
+INT_DP_CASES += [("runs-%s%s" % (c, "-fixed" if it == 0 else ""), d, s, e, it)
+                 for name in ("full", "step", "dict") for c, d, s, e in run_list_fixtures.cases(name) for it in (5, 0)]
 
 
 @pytest.mark.parametrize("name,data,s,e,iters", INT_DP_CASES, ids=[c[0] for c in INT_DP_CASES])
@@ -149,7 +155,7 @@ def test_integer_dp_model_equals_reference_dp(name, data, s, e, iters):
     steps_total, steps_int = int(out[0]), int(out[1])
     assert mism == 0
     assert steps_total > 0
-    if name in ("text", "random"):
+    if name in ("text", "random") or name.startswith("runs-"):
         assert steps_int > 0.8 * steps_total   # the model really ran in the integer representation
 
 

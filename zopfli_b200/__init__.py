@@ -41,7 +41,7 @@ class Stats(C.Structure):
                 ("ms_split", C.c_double), ("split_evals", C.c_uint64), ("split_rounds", C.c_uint64),
                 ("iterate_launches", C.c_uint64), ("int_steps", C.c_uint64),
                 ("dp_cyc_sum", C.c_uint64 * 5), ("dp_cnt_sum", C.c_uint64 * 6),
-                ("dp_cyc_max", C.c_uint64 * 5), ("dp_cnt_max", C.c_uint64 * 6)]
+                ("dp_cyc_max", C.c_uint64 * 5), ("dp_cnt_max", C.c_uint64 * 6), ("ovf_regrows", C.c_uint64)]
 
     def as_dict(self):
         return {n: (list(getattr(self, n)) if n.startswith(("cyc_", "dp_c")) else getattr(self, n)) for n, _ in self._fields_}

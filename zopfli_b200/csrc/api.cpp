@@ -996,6 +996,7 @@ void ZopfliB200GetStats(ZopfliB200Stats* o) {
   o->iterate_steps = e.iterate_steps; o->h2d_bytes = e.h2d_bytes; o->d2h_bytes = e.d2h_bytes;
   for (int k = 0; k < 6; k++) { o->cyc_sum[k] = e.cyc_sum[k]; o->cyc_max[k] = e.cyc_max[k]; }
   o->max_block_positions = e.max_block_positions;
+  o->ovf_regrows = e.ovf_regrows;
   o->ms_split = e.ms_split; o->split_evals = e.split_evals; o->split_rounds = e.split_rounds;
   o->iterate_launches = e.iterate_launches;
   o->int_steps = e.int_steps;

@@ -699,6 +699,7 @@ EngineStats Engine::stats_all() {
     r.iterate_launches += a.iterate_launches;
     r.launches += a.launches; r.match_positions += a.match_positions; r.iterate_positions += a.iterate_positions;
     r.iterate_steps += a.iterate_steps; r.h2d_bytes += a.h2d_bytes; r.d2h_bytes += a.d2h_bytes; r.int_steps += a.int_steps;
+    r.ovf_regrows += a.ovf_regrows;
     uint64_t ta = 0, tr = 0;
     for (int i = 0; i < 6; i++) { r.cyc_sum[i] += a.cyc_sum[i]; ta += a.cyc_max[i]; tr += r.cyc_max[i]; }
     for (int i = 0; i < 5; i++) r.dp_cyc_sum[i] += a.dp_cyc_sum[i];
@@ -729,6 +730,7 @@ EngineStats Engine::stats() {
     r.iterate_launches += a.iterate_launches;
     r.launches += a.launches; r.match_positions += a.match_positions; r.iterate_positions += a.iterate_positions;
     r.iterate_steps += a.iterate_steps; r.h2d_bytes += a.h2d_bytes; r.d2h_bytes += a.d2h_bytes; r.int_steps += a.int_steps;
+    r.ovf_regrows += a.ovf_regrows;
     uint64_t ta = 0, tr = 0;
     for (int i = 0; i < 6; i++) { r.cyc_sum[i] += a.cyc_sum[i]; ta += a.cyc_max[i]; tr += r.cyc_max[i]; }
     for (int i = 0; i < 5; i++) r.dp_cyc_sum[i] += a.dp_cyc_sum[i];
@@ -955,6 +957,7 @@ void Engine::parse_common(const std::vector<ParseRange>& ranges, ParseResult& ou
     l.sync();
     if (L.any_parse && counters.ovf_used > l.ovf_cap) {  // run-list overflow arena too small: grow, redo
       l.ovf_cap = Impl::grown_ovf_cap(counters.ovf_used);
+      l.acc.ovf_regrows++;
       if (attempt > 2) { fprintf(stderr, "zopfli-b200: overflow arena did not converge\n"); abort(); }
       continue;
     }
@@ -1023,7 +1026,12 @@ void Engine::match_table(uint64_t instart, uint64_t inend, std::vector<uint16_t>
     CK(cudaMemcpyAsync(&c, l.counters.p, sizeof(c), cudaMemcpyDeviceToHost, l.stream));
     l.sync();
     const size_t used = c.ovf_used;
-    if (used > l.ovf_cap) { l.ovf_cap = Impl::grown_ovf_cap(used); if (attempt > 2) abort(); continue; }
+    if (used > l.ovf_cap) {
+      l.ovf_cap = Impl::grown_ovf_cap(used);
+      l.acc.ovf_regrows++;
+      if (attempt > 2) abort();
+      continue;
+    }
     h_ld.resize(n); h_runs.resize(n * kRunSlots); h_mlen.resize(n); h_ovf.resize(used + 1);
     h_hv.resize(L.nkeys); h_hv2.resize(L.nkeys); h_same.resize(n);
     if (n) {
