@@ -302,6 +302,7 @@ typedef struct ZopfliB200Stats {
   uint64_t dp_cyc_sum[5], dp_cnt_sum[6];                 /* DP cycles / groups of 32 steps by kind: integer window, fp64 magic, fp64 plain, */
   uint64_t dp_cyc_max[5], dp_cnt_max[6];                 /* fp64 ring-joining, general; cnt[5] = positions in the per-step loop; sum over blocks / critical block */
   uint64_t ovf_regrows;                                  /* batches redone because their run lists outgrew the overflow arena */
+  uint64_t log_regrows;                                  /* batches redone because a statistics sum outgrew the log table */
 } ZopfliB200Stats;
 void ZopfliB200GetStats(ZopfliB200Stats* out);
 void ZopfliB200ResetStats(void);

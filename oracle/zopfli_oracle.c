@@ -741,8 +741,32 @@ static void randomize_freqs(ZoRan* s, size_t* freqs, int n) { /* squeeze.c:96-10
     if ((ran(s) >> 4) % 3 == 0) freqs[i] = freqs[ran(s) % (unsigned)n];
 }
 
+/* the largest sum of either statistics array, and the largest single count, that calc_statistics takes: how far
+ * the log table of an implementation that looks up log(n) must reach (the blend and RandomizeFreqs can take the
+ * sum past twice the block's symbols) */
+static void note_stats(const ZoStats* st, size_t* max_sum, size_t* max_count) {
+  size_t sl = 0, sd = 0;
+  int k;
+  if (!max_sum) return;
+  for (k = 0; k < ZO_NUM_LL; k++) {
+    sl += st->litlens[k];
+    if (st->litlens[k] > *max_count) *max_count = st->litlens[k];
+  }
+  for (k = 0; k < ZO_NUM_D; k++) {
+    sd += st->dists[k];
+    if (st->dists[k] > *max_count) *max_count = st->dists[k];
+  }
+  if (sl > *max_sum) *max_sum = sl;
+  if (sd > *max_sum) *max_sum = sd;
+}
+
 void zo_lz77_optimal(const uint8_t* in, size_t instart, size_t inend, int numiterations,
                      ZoStore* out) {
+  zo_lz77_optimal_stats(in, instart, inend, numiterations, out, NULL, NULL);
+}
+
+void zo_lz77_optimal_stats(const uint8_t* in, size_t instart, size_t inend, int numiterations,
+                           ZoStore* out, size_t* max_sum, size_t* max_count) {
   size_t nb = inend - instart;
   ZoSegment* seg;
   ZoTable tab;
@@ -754,6 +778,7 @@ void zo_lz77_optimal(const uint8_t* in, size_t instart, size_t inend, int numite
   ZoRan rs = {1, 2}; /* squeeze.c:85-88 */
   int lastrandomstep = -1, i;
   out->size = 0;
+  if (max_sum) *max_sum = *max_count = 0;
   if (nb == 0) return;
   seg = zo_segment_new(in, instart, inend);
   table_build(seg, &tab);
@@ -764,6 +789,7 @@ void zo_lz77_optimal(const uint8_t* in, size_t instart, size_t inend, int numite
   memset(&beststats, 0, sizeof(beststats));
   greedy_segment(seg, &current); /* squeeze.c:481 */
   get_statistics(&current, &stats);
+  note_stats(&stats, max_sum, max_count);
   for (i = 0; i < numiterations; i++) { /* squeeze.c:486-519 */
     size_t llc[ZO_NUM_LL], dc[ZO_NUM_D];
     int k;
@@ -781,6 +807,7 @@ void zo_lz77_optimal(const uint8_t* in, size_t instart, size_t inend, int numite
     memset(stats.litlens, 0, sizeof(stats.litlens));
     memset(stats.dists, 0, sizeof(stats.dists));
     get_statistics(&current, &stats);
+    note_stats(&stats, max_sum, max_count);
     if (lastrandomstep != -1) { /* squeeze.c:505-511, AddWeighedStatFreqs :65-78 */
       for (k = 0; k < ZO_NUM_LL; k++)
         stats.litlens[k] = (size_t)(stats.litlens[k] * 1.0 + laststats.litlens[k] * 0.5);
@@ -788,6 +815,7 @@ void zo_lz77_optimal(const uint8_t* in, size_t instart, size_t inend, int numite
         stats.dists[k] = (size_t)(stats.dists[k] * 1.0 + laststats.dists[k] * 0.5);
       stats.litlens[256] = 1;
       calc_statistics(&stats);
+      note_stats(&stats, max_sum, max_count);
     }
     if (i > 5 && cost == lastcost) { /* squeeze.c:512-517 */
       stats = beststats;
@@ -795,6 +823,7 @@ void zo_lz77_optimal(const uint8_t* in, size_t instart, size_t inend, int numite
       randomize_freqs(&rs, stats.dists, ZO_NUM_D);
       stats.litlens[256] = 1;
       calc_statistics(&stats);
+      note_stats(&stats, max_sum, max_count);
       lastrandomstep = i;
     }
     lastcost = cost;

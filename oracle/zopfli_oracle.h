@@ -60,6 +60,9 @@ void zo_lz77_greedy(const uint8_t* in, size_t instart, size_t inend, ZoStore* ou
 /* ZopfliLZ77Optimal (squeeze.c:446-526) / ZopfliLZ77OptimalFixed (squeeze.c:528-560). */
 void zo_lz77_optimal(const uint8_t* in, size_t instart, size_t inend, int numiterations,
                      ZoStore* out);
+/* the same, and the largest statistics sum and count it hands to the entropy (max_sum and max_count are both NULL or both set) */
+void zo_lz77_optimal_stats(const uint8_t* in, size_t instart, size_t inend, int numiterations,
+                           ZoStore* out, size_t* max_sum, size_t* max_count);
 void zo_lz77_optimal_fixed(const uint8_t* in, size_t instart, size_t inend, ZoStore* out);
 
 /* ZopfliLengthLimitedCodeLengths (katajainen.c:172-262), restated as the classic

@@ -10,6 +10,7 @@ import os
 import numpy as np
 import pytest
 
+import random_step_fixtures
 import run_list_fixtures
 import zref
 from zopfli_b200 import corpus
@@ -61,6 +62,17 @@ def test_limited_walk_is_table_lookup(ref, oracle, name, data, s, e):
     j = np.nonzero(limits >= 3)[0]
     assert np.array_equal(rl[j], limits[j])
     assert np.array_equal(rd[j], sub[j, limits[j]])
+
+
+# random restarts and blended statistics (random_step_fixtures.py), each at its own iteration count
+RANDOM_STEP_CASES = [c for c in random_step_fixtures.all_cases() if c[0] in random_step_fixtures.SMALL]
+
+
+@pytest.mark.parametrize("name,call,data,s,e,iters", RANDOM_STEP_CASES, ids=[c[0] for c in RANDOM_STEP_CASES])
+def test_store_seam_at_random_steps(ref, oracle, name, call, data, s, e, iters):
+    a = ref.lz77(data, s, e, 0, iters)
+    b = oracle.lz77(data, s, e, 0, iters)
+    assert np.array_equal(a[0], b[0]) and np.array_equal(a[1], b[1])
 
 
 @pytest.mark.parametrize("name,data,s,e", CASES, ids=[c[0] for c in CASES])

@@ -288,6 +288,9 @@ class Oracle:
             getattr(L, f).argtypes = [C.c_void_p, C.c_size_t, C.c_size_t, C.POINTER(ZoStore)]
         L.zo_lz77_optimal.restype = None
         L.zo_lz77_optimal.argtypes = [C.c_void_p, C.c_size_t, C.c_size_t, C.c_int, C.POINTER(ZoStore)]
+        L.zo_lz77_optimal_stats.restype = None
+        L.zo_lz77_optimal_stats.argtypes = [C.c_void_p, C.c_size_t, C.c_size_t, C.c_int, C.POINTER(ZoStore),
+                                            C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]
         L.zo_store_init.argtypes = [C.POINTER(ZoStore)]
         L.zo_store_free.argtypes = [C.POINTER(ZoStore)]
         L.zo_length_limited_code_lengths.restype = C.c_int
@@ -316,6 +319,20 @@ class Oracle:
         if mode == 1:
             return self._store_call(self.lib.zo_lz77_optimal_fixed, a.ctypes.data, instart, inend)
         return self._store_call(self.lib.zo_lz77_greedy, a.ctypes.data, instart, inend)
+
+    def lz77_stats(self, data, instart, inend, numiterations):
+        """the optimal store, and the largest statistics sum and count the iterations hand to the entropy"""
+        a = _np_u8(data)
+        ms, mc = C.c_size_t(0), C.c_size_t(0)
+        st = ZoStore()
+        self.lib.zo_store_init(C.byref(st))
+        self.lib.zo_lz77_optimal_stats(a.ctypes.data, instart, inend, numiterations, C.byref(st), C.byref(ms),
+                                       C.byref(mc))
+        n = st.size
+        ll = np.ctypeslib.as_array(st.litlens, (n,)).copy() if n else np.zeros(0, np.uint16)
+        dd = np.ctypeslib.as_array(st.dists, (n,)).copy() if n else np.zeros(0, np.uint16)
+        self.lib.zo_store_free(C.byref(st))
+        return ll, dd, ms.value, mc.value
 
     def match_table(self, data, instart, inend, want_sublen=True):
         a = _np_u8(data)

@@ -997,6 +997,7 @@ void ZopfliB200GetStats(ZopfliB200Stats* o) {
   for (int k = 0; k < 6; k++) { o->cyc_sum[k] = e.cyc_sum[k]; o->cyc_max[k] = e.cyc_max[k]; }
   o->max_block_positions = e.max_block_positions;
   o->ovf_regrows = e.ovf_regrows;
+  o->log_regrows = e.log_regrows;
   o->ms_split = e.ms_split; o->split_evals = e.split_evals; o->split_rounds = e.split_rounds;
   o->iterate_launches = e.iterate_launches;
   o->int_steps = e.int_steps;

@@ -132,10 +132,12 @@ struct LogService {
   ~LogService() {
     if (filler.joinable()) filler.join();
   }
-  // table with at least need_n entries on `device`.  The default 2^21 entries cover every count a master
-  // block can produce (symbols <= 10^6, blended statistics < 2x that); larger single ranges
-  // (ZopfliDeflatePart with block splitting off) grow the table on demand.  An outgrown device copy is
-  // left allocated: other contexts may still be reading it.
+  // table with at least need_n entries on `device`.  No fixed size covers every statistics sum: the blend
+  // (squeeze.c:505-511) adds half the previous statistics, and RandomizeFreqs copies counts between entries, so
+  // the sum the entropy takes can exceed twice the block's symbols (2.2x has been seen on random data).  The
+  // default 2^21 entries and parse_common's 2 x positions pre-size cover the usual case; a batch that still
+  // meets a sum past the table grows it here and is redone.  An outgrown device copy is left allocated: other
+  // contexts may still be reading it.
   const double* get(int device, cudaStream_t st, uint32_t need_n, uint32_t* have_n) {
     std::lock_guard<std::mutex> g(mu);
     if (!joined) { filler.join(); joined = true; }
@@ -699,7 +701,7 @@ EngineStats Engine::stats_all() {
     r.iterate_launches += a.iterate_launches;
     r.launches += a.launches; r.match_positions += a.match_positions; r.iterate_positions += a.iterate_positions;
     r.iterate_steps += a.iterate_steps; r.h2d_bytes += a.h2d_bytes; r.d2h_bytes += a.d2h_bytes; r.int_steps += a.int_steps;
-    r.ovf_regrows += a.ovf_regrows;
+    r.ovf_regrows += a.ovf_regrows; r.log_regrows += a.log_regrows;
     uint64_t ta = 0, tr = 0;
     for (int i = 0; i < 6; i++) { r.cyc_sum[i] += a.cyc_sum[i]; ta += a.cyc_max[i]; tr += r.cyc_max[i]; }
     for (int i = 0; i < 5; i++) r.dp_cyc_sum[i] += a.dp_cyc_sum[i];
@@ -730,7 +732,7 @@ EngineStats Engine::stats() {
     r.iterate_launches += a.iterate_launches;
     r.launches += a.launches; r.match_positions += a.match_positions; r.iterate_positions += a.iterate_positions;
     r.iterate_steps += a.iterate_steps; r.h2d_bytes += a.h2d_bytes; r.d2h_bytes += a.d2h_bytes; r.int_steps += a.int_steps;
-    r.ovf_regrows += a.ovf_regrows;
+    r.ovf_regrows += a.ovf_regrows; r.log_regrows += a.log_regrows;
     uint64_t ta = 0, tr = 0;
     for (int i = 0; i < 6; i++) { r.cyc_sum[i] += a.cyc_sum[i]; ta += a.cyc_max[i]; tr += r.cyc_max[i]; }
     for (int i = 0; i < 5; i++) r.dp_cyc_sum[i] += a.dp_cyc_sum[i];
@@ -884,7 +886,8 @@ void Engine::parse_common(const std::vector<ParseRange>& ranges, ParseResult& ou
   m.build_layout(ranges, L);
   std::vector<JobState> js(ns);
   Counters counters{};
-  {  // statistics counts stay below 2 x symbols (blended statistics, squeeze.c:70-75): size the log table for it
+  {  // statistics sums usually stay below 2 x symbols; a blended or randomized sum past that is met below: the log
+     // table is grown to it and the batch redone
     uint64_t need = 0;
     for (const SegDesc& sg : L.segs)
       if (sg.mode == 1) need = std::max<uint64_t>(need, 2ull * sg.npos + 16);
@@ -961,6 +964,22 @@ void Engine::parse_common(const std::vector<ParseRange>& ranges, ParseResult& ou
       if (attempt > 2) { fprintf(stderr, "zopfli-b200: overflow arena did not converge\n"); abort(); }
       continue;
     }
+    uint32_t log_miss = 0;  // the largest statistics count or sum whose log fell outside the table
+    for (size_t i = 0; i < ns; i++)
+      if (js[i].flags & 1) log_miss = std::max(log_miss, js[i].log_miss);
+    if (log_miss) {  // a statistics sum outgrew the log table: grow it past that sum with room to spare, redo
+      if (log_miss >= 0xfffffff0u) {
+        fprintf(stderr, "zopfli-b200: symbol count %u beyond the largest log table\n", log_miss);
+        abort();
+      }
+      {
+        std::lock_guard<std::mutex> g(m.mu);
+        m.log_need = std::max<uint32_t>(m.log_need, (uint32_t)std::min<uint64_t>(log_miss + (uint64_t)log_miss / 4 + 1024, 0xfffffff0ull));
+      }
+      l.acc.log_regrows++;
+      if (attempt > 2) { fprintf(stderr, "zopfli-b200: log table did not converge\n"); abort(); }
+      continue;
+    }
     const uint32_t total = dest < 0 ? counters.out_used : 0u;
     out.ll.resize(total);
     out.d.resize(total);
@@ -981,11 +1000,6 @@ void Engine::parse_common(const std::vector<ParseRange>& ranges, ParseResult& ou
     out.cost[i] = js[i].best_cost;
     if (!greedy_only && ranges[i].mode == 0) {
       fprintf(stderr, "zopfli-b200: greedy and optimal ranges cannot share a batch\n");
-      abort();
-    }
-    if (js[i].flags & 1) {
-      fprintf(stderr, "zopfli-b200: symbol count beyond the %u-entry log table in block %zu (iteration %u)\n",
-              m.logtab_n, i, js[i].iters_done);
       abort();
     }
     if (js[i].flags & 2) { fprintf(stderr, "zopfli-b200: corrupted length chain in block %zu\n", i); abort(); }

@@ -33,6 +33,7 @@ struct EngineStats {  // accumulated since the last reset; times from CUDA event
   uint64_t dp_cyc_sum[5], dp_cnt_sum[6];   // DP cycles / groups by kind of group (JobState::dpc, dpn), summed over blocks
   uint64_t dp_cyc_max[5], dp_cnt_max[6];   // same for the critical-path block
   uint64_t ovf_regrows;  // batches redone because their run lists outgrew the overflow arena
+  uint64_t log_regrows;  // batches redone because a statistics sum outgrew the log table
 };
 
 class Engine {

@@ -204,27 +204,27 @@ __device__ __forceinline__ double warp_min_first(double v, int& idx) {
   return v;
 }
 
-// ZopfliCalculateEntropy tree.c:71-94 over n counts (n = 288 or 32). Returns false if a count or
-// the sum falls outside the host-provided log table.
-__device__ bool warp_entropy(const uint32_t* cnt, int n, double* out, const Batch& b, uint32_t lane) {
+// ZopfliCalculateEntropy tree.c:71-94 over n counts (n = 288 or 32). Returns 0, or the largest count or
+// sum that falls outside the host-provided log table.
+__device__ uint32_t warp_entropy(const uint32_t* cnt, int n, double* out, const Batch& b, uint32_t lane) {
   uint32_t sum = 0;
   for (int i = lane; i < n; i += 32) sum += cnt[i];
 #pragma unroll
   for (int d = 16; d > 0; d >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, d);
   uint32_t si = sum == 0 ? (uint32_t)n : sum;
-  bool ok = si < b.logtab_n;
-  double log2sum = ok ? b.logtab[si] : 0.0;
+  uint32_t miss = si < b.logtab_n ? 0u : si;
+  double log2sum = miss ? 0.0 : b.logtab[si];
   for (int i = lane; i < n; i += 32) {
     uint32_t c = cnt[i];
     double v = log2sum;
     if (c) {
       if (c < b.logtab_n) v = log2sum - b.logtab[c];
-      else ok = false;
+      else miss = max(miss, c);
     }
     if (v < 0 && v > -1e-5) v = 0;  // tree.c:91
     out[i] = v;
   }
-  return __all_sync(0xffffffffu, ok);
+  return __reduce_max_sync(0xffffffffu, miss);
 }
 
 // ---- ZopfliLengthLimitedCodeLengths (katajainen.c:172-262) by the whole warp ----
@@ -842,7 +842,7 @@ __global__ void __launch_bounds__(NW * 32, NW == 2 ? 4 : 1) k_iterate(Batch b, c
   const uint8_t* dsx_g = b.dsx + sd.pos_off * 32;
   const bool fixed = sd.mode == 2;
   int curbuf = 0, bestbuf = 1;
-  uint32_t flags = 0;
+  uint32_t flags = 0, log_miss = 0;  // log_miss: warp_entropy's value past the log table (flags bit 0)
   if (threadIdx.x == 0) {
     for (int i = 0; i < 4; i++) { mbar_init(&s.full[i], 1); mbar_init(&s.empty[i], 1); dyn.tag[i] = 0; dyn.xchi[i] = kIntInf; }
     dyn.gen = 0;
@@ -958,9 +958,8 @@ __global__ void __launch_bounds__(NW * 32, NW == 2 ? 4 : 1) k_iterate(Batch b, c
     __syncwarp();
     if (lane == 0) s.stats[256] = 1;  // squeeze.c:409
     __syncwarp();
-    bool ok = warp_entropy(s.stats, kNumLL, s.llcost, b, lane);
-    ok &= warp_entropy(s.stats + 288, kNumD, s.dcost, b, lane);
-    if (!ok) flags |= 1;
+    log_miss = max(warp_entropy(s.stats, kNumLL, s.llcost, b, lane), warp_entropy(s.stats + 288, kNumD, s.dcost, b, lane));
+    if (log_miss) flags |= 1;
   } else {
     for (int i = lane; i < kNumLL; i += 32) s.llcost[i] = (double)fixed_ll_length(i);
     if (lane < kNumD) s.dcost[lane] = 5.0;
@@ -1707,9 +1706,8 @@ __global__ void __launch_bounds__(NW * 32, NW == 2 ? 4 : 1) k_iterate(Batch b, c
       lastrandomstep = it;
     }
     if (need_entropy) {
-      bool ok = warp_entropy(s.stats, kNumLL, s.llcost, b, lane);
-      ok &= warp_entropy(s.stats + 288, kNumD, s.dcost, b, lane);
-      if (!ok) flags |= 1;
+      log_miss = max(warp_entropy(s.stats, kNumLL, s.llcost, b, lane), warp_entropy(s.stats + 288, kNumD, s.dcost, b, lane));
+      if (log_miss) flags |= 1;
       __syncwarp();
     }
     lastcost = cost;
@@ -1728,6 +1726,7 @@ __global__ void __launch_bounds__(NW * 32, NW == 2 ? 4 : 1) k_iterate(Batch b, c
     js->flags = flags;
     js->iters_done = (uint32_t)it;
     js->int_groups = igroups;
+    js->log_miss = log_miss;
     for (int i = 0; i < 5; i++) js->dpc[i] = s.dpc[i];
     for (int i = 0; i < 6; i++) js->dpn[i] = s.dpn[i];
   }

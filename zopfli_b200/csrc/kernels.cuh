@@ -85,7 +85,7 @@ struct JobState {   // per segment, written by k_greedy / k_iterate
   uint32_t flags;        // bit0: log table overflow (needs host assistance)
   uint32_t iters_done;
   uint32_t int_groups;   // groups of 32 DP steps that ran in the integer window (all iterations)
-  uint32_t pad_;
+  uint32_t log_miss;     // with flags bit 0: the value whose log fell outside the table (the host grows it past it)
   uint64_t best_cost;
   uint64_t cyc[6];       // SM cycles spent in: model, DP, trace, follow, block cost, statistics
   uint64_t dpc[5];       // DP cycles by kind of group: integer window, fp64 fast (magic / plain / ring-joining), general
