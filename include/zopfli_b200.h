@@ -169,7 +169,7 @@ int ZopfliB200Adler32Device(const unsigned char* dev_in, size_t size, void* cuda
  * on its bytes, the 32 KiB before it and whether it is the last one, so the compressor runs the input as waves
  * of whole master blocks (half as many as ZopfliCompress runs at once on the device, so that the two waves in
  * flight fit the device memory of one call: about 72 on an 80 GB card by the driver's schedule; ZOPFLI_B200_BATCH and ZOPFLI_B200_CHUNKS shrink them) while more bytes arrive.
- *  - Identical bytes: without a flush or a dictionary (below), every Write output followed by the Finish
+ *  - Identical bytes: without a flush, a dictionary or restart points (below), every Write output followed by the Finish
  *    output, concatenated, equals ZopfliCompress(options, output_type, <all chunks concatenated>), for every
  *    chunking (zero-length writes included) and all three formats.  A compressor finished at once gives
  *    ZopfliCompress of an empty input.
@@ -249,6 +249,40 @@ int ZopfliB200CompressorSetDictionary(ZopfliB200Compressor* c, const unsigned ch
  * (all that is left, not final; 0 when handed == received). */
 int ZopfliB200CompressorWave(size_t received, int finished, size_t handed, size_t wave_blocks, size_t* a, size_t* b,
                              int* final);
+/* Restart points: a full flush every `interval` bytes of data, made inside the waves.
+ * Byte contract.  An interval N >= 1 means a full flush at every data position k*N (k >= 1) that has at least one
+ * data byte after it: X position d + k*N with a dictionary of d bytes.  The automatic flush at k*N happens once
+ * byte k*N + 1 has arrived, and never at the end of the data, where Finish comes instead.  The stream is exactly
+ * the one the contract above defines for the caller's flushes plus (k*N, FULL) for every such k, merged by
+ * position; at equal positions the caller's flush comes first (it was called before the byte past it arrived),
+ * so a Flush(FULL) at k*N yields two markers.  Without an interval nothing changes.
+ * Segments cut at restart points share waves: a wave is still wave_blocks units, a unit being a master block of
+ * a segment (counted from the segment's start), and every unit's parse sees no byte before the last full flush
+ * at or before it.  So an interval below 1e6 makes waves shorter in bytes, not fewer in units; the staging bound
+ * and the two waves in flight stay as they are.
+ * SetRestartInterval is accepted once, before the first Write or Flush call of any length, and combines with
+ * SetDictionary and with explicit flushes.  It returns nonzero, nothing changed, for a NULL c, interval 0, a
+ * second call, a call after the first Write or Flush, and a call after Finish.
+ * RestartPoints lists one entry per full flush, automatic or explicit, in stream order: data_off is the data
+ * position of the flush, stream_off the offset of the first byte after its marker, counted from the first byte
+ * the compressor returned (header included).  Raw inflate of the stream from stream_off on (zlib wbits -15)
+ * yields data[data_off:], in all three formats.  An entry is listed once its marker's bytes have been returned;
+ * after Finish the list is complete.  The start of the stream is not an entry: a reader whose target lies before
+ * the first entry decodes from the start, with the dictionary if there is one.  Returns the number of entries and
+ * writes min(count, cap) of them; either array may be NULL.  Returns 0 for a NULL c.
+ * After Finish, ZopfliB200LastMasterBitOffsets gives every master block of every segment, then the end; markers
+ * are not entries. */
+int ZopfliB200CompressorSetRestartInterval(ZopfliB200Compressor* c, size_t interval);
+size_t ZopfliB200CompressorRestartPoints(ZopfliB200Compressor* c, uint64_t* data_off, uint64_t* stream_off, size_t cap);
+/* The compressor's schedule with restart points as a pure function (csrc/dist_layout.hpp next_wave; no GPU
+ * needed): as ZopfliB200CompressorWave, with `floor` the last full flush at or before `handed` and restart points at
+ * dict_len + k*interval (interval 0: none).  Returns the number of units of the next wave (0: no wave is ready)
+ * and writes min(count, cap) of them: unit i is bytes [a[i], b[i]) parsed seeing no byte before floors[i], and
+ * restart[i] is 1 where the automatic full flush's marker follows it.  *final is the wave's BFINAL.  Any of the
+ * arrays and final may be NULL. */
+size_t ZopfliB200CompressorWaveUnits(size_t received, int finished, size_t handed, size_t floor, size_t dict_len,
+                                     size_t interval, size_t wave_blocks, size_t* a, size_t* b, size_t* floors,
+                                     int* restart, size_t cap, int* final);
 
 /* ---- several GPUs, one stream (SURVEY 8(e)) ----
  * The master blocks of one input (the reference's independent unit, deflate.c:908-931) are sharded

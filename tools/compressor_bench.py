@@ -11,7 +11,13 @@ With --flush-every BYTES, two more legs (host and device chunks, 64 MiB writes) 
 input: each flush runs what has arrived as a wave of its own, however short.  Their output differs from
 ZopfliCompress's by the flush points, so it is checked by inflating it instead.
 
+With --restart-every BYTES, two more legs (host chunks, 64 MiB writes) put a full flush every BYTES of input: one
+calls Flush(FULL) at each point, so each point ends a wave of its own; the other sets restart_interval=BYTES, so
+the segments between points share waves.  Their streams must be byte-identical ("identical_to_explicit"), and
+every index entry of the restart leg must inflate raw to the data from its offset on.
+
     python tools/compressor_bench.py [--mib 430] [--reps 3] [--numiterations 15] [--flush-every BYTES]
+                                     [--restart-every BYTES]
 """
 import argparse
 import json
@@ -44,9 +50,11 @@ def run_whole(lib, data, kw):
     return lib.compress_ptr(a.ctypes.data, len(data), zb.ZOPFLI_FORMAT_GZIP, **kw)
 
 
-def run_pieces(lib, src, write, kw, device, flush_every=0):
+def run_pieces(lib, src, write, kw, device, flush_every=0, mode=zlib.Z_SYNC_FLUSH, restart_interval=None,
+               index=None):
     out = []
-    with lib.compressobj(zb.ZOPFLI_FORMAT_GZIP, device=0 if device else None, **kw) as c:
+    with lib.compressobj(zb.ZOPFLI_FORMAT_GZIP, device=0 if device else None, restart_interval=restart_interval,
+                         **kw) as c:
         p = 0
         while p < len(src):
             q = min(p + write, len(src))
@@ -54,10 +62,18 @@ def run_pieces(lib, src, write, kw, device, flush_every=0):
                 q = min(q, (p // flush_every + 1) * flush_every)
             out.append(c.compress(src[p:q]))
             p = q
-            if flush_every and p % flush_every == 0:
-                out.append(c.flush(zlib.Z_SYNC_FLUSH))
+            # a full flush only where data follows, as restart points are placed
+            if flush_every and p % flush_every == 0 and (mode == zlib.Z_SYNC_FLUSH or p < len(src)):
+                out.append(c.flush(mode))
         out.append(c.flush())
+        if index is not None:
+            index[:] = c.restart_points()
     return b"".join(out)
+
+
+def index_inflates(stream, data, index):
+    """every entry's first 64 KiB inflate raw to the data from its offset on"""
+    return all(zlib.decompressobj(-15).decompress(stream[s:], 65536) == data[d:d + 65536] for d, s in index)
 
 
 def main():
@@ -66,6 +82,8 @@ def main():
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--numiterations", type=int, default=15)
     ap.add_argument("--flush-every", type=int, default=0, help="bytes of input between sync flushes (0: no flush legs)")
+    ap.add_argument("--restart-every", type=int, default=0,
+                    help="bytes of input between full flushes, explicit and by restart_interval (0: no restart legs)")
     args = ap.parse_args()
     kw = {"numiterations": args.numiterations}
     lib = zb.library()
@@ -86,7 +104,14 @@ def main():
                      lambda: run_pieces(lib, host_view, 64 * MIB, kw, False, f)))
         legs.append(("compressor device 64 MiB, sync flush every %d B" % f,
                      lambda: run_pieces(lib, dev, 64 * MIB, kw, True, f)))
-    want = None
+    r = args.restart_every
+    index = []
+    if r:
+        legs.append(("compressor host 64 MiB, Flush(FULL) every %d B" % r,
+                     lambda: run_pieces(lib, host_view, 64 * MIB, kw, False, r, zlib.Z_FULL_FLUSH)))
+        legs.append(("compressor host 64 MiB, restart_interval=%d" % r,
+                     lambda: run_pieces(lib, host_view, 64 * MIB, kw, False, restart_interval=r, index=index)))
+    want, explicit = None, None
     for rep in range(args.reps):
         for name, fn in legs:
             torch.cuda.synchronize()
@@ -99,7 +124,14 @@ def main():
             free, total = torch.cuda.mem_get_info(0)
             rec = {"rep": rep, "leg": name, "ms": round(ms, 1), "MiB_s": round(len(data) / MIB / (ms / 1e3), 2),
                    "out_bytes": len(got)}
-            if "flush" in name:
+            if "Flush(FULL)" in name:
+                explicit = got
+                rec["inflates"] = zlib.decompress(got, 31) == data
+            elif "restart_interval" in name:
+                rec["identical_to_explicit"] = got == explicit
+                rec["restart_points"] = len(index)
+                rec["index_inflates"] = index_inflates(got, data, index)
+            elif "flush" in name:
                 rec["inflates"] = zlib.decompress(got, 31) == data
             else:
                 rec["identical"] = got == want

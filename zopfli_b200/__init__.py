@@ -60,7 +60,8 @@ EXPORTS = ["ZopfliInitOptions", "ZopfliCompress", "ZopfliDeflate", "ZopfliDeflat
            "ZopfliB200Version", "ZopfliB200CompressDeviceToDevice", "ZopfliB200FreeDevice", "ZopfliB200Crc32Device",
            "ZopfliB200Adler32Device", "ZopfliB200HostChecksumSliced", "ZopfliB200CompressorNew", "ZopfliB200CompressorWrite",
            "ZopfliB200CompressorFinish", "ZopfliB200CompressorFree", "ZopfliB200CompressorWave",
-           "ZopfliB200CompressorFlush", "ZopfliB200CompressorSetDictionary"]
+           "ZopfliB200CompressorFlush", "ZopfliB200CompressorSetDictionary", "ZopfliB200CompressorSetRestartInterval",
+           "ZopfliB200CompressorRestartPoints", "ZopfliB200CompressorWaveUnits"]
 
 
 def _pad(data):
@@ -219,6 +220,12 @@ class Library:
         L.ZopfliB200CompressorFree.restype = None
         L.ZopfliB200CompressorWave.argtypes = [sz, C.c_int, sz, sz, C.POINTER(sz), C.POINTER(sz), C.POINTER(C.c_int)]
         L.ZopfliB200CompressorWave.restype = C.c_int
+        L.ZopfliB200CompressorSetRestartInterval.argtypes = [vp, sz]
+        L.ZopfliB200CompressorSetRestartInterval.restype = C.c_int
+        L.ZopfliB200CompressorRestartPoints.argtypes = [vp, vp, vp, sz]
+        L.ZopfliB200CompressorRestartPoints.restype = sz
+        L.ZopfliB200CompressorWaveUnits.argtypes = [sz, C.c_int, sz, sz, sz, sz, sz, vp, vp, vp, vp, sz, C.POINTER(C.c_int)]
+        L.ZopfliB200CompressorWaveUnits.restype = sz
         # device-resident calls and the device emission seam (csrc/device_api.cpp); a host-only test build of the
         # ABI does not export them
         for name, args, res in (("ZopfliB200CompressDeviceToDevice",
@@ -530,15 +537,18 @@ class Library:
         return self._device_checksum(self.lib.ZopfliB200Adler32Device, t, stream)
 
     # ---- input in pieces (ZopfliB200Compressor) ----
-    def compressobj(self, fmt=ZOPFLI_FORMAT_GZIP, device=None, stream=None, zdict=None, **kw) -> "Compressor":
+    def compressobj(self, fmt=ZOPFLI_FORMAT_GZIP, device=None, stream=None, zdict=None, restart_interval=None,
+                    **kw) -> "Compressor":
         """A compressor shaped like zlib.compressobj: compress(chunk) -> bytes, flush(mode) -> bytes.  Without
         zdict and sync / full flushes, all outputs concatenated equal compress(<all chunks>, fmt, **kw).
         device=None: chunks are bytes-like objects; device=<index or torch.device>: chunks are contiguous CUDA
         tensors of that device, each copied after the work queued on `stream`, or, without stream=, on the
         tensor's current stream (a private stream of the compressor waits for it, so the caller's streams gain
         no dependency).  zdict: a preset dictionary (zlib and raw deflate only), bytes-like, or for a device
-        compressor also a contiguous uint8 CUDA tensor of its device."""
-        return Compressor(self, fmt, device, stream, zdict, **kw)
+        compressor also a contiguous uint8 CUDA tensor of its device.  restart_interval=N: a full flush at every
+        N bytes of data that has a byte after it, compressed inside the waves; Compressor.restart_points() is the
+        index of where raw inflating can start."""
+        return Compressor(self, fmt, device, stream, zdict, restart_interval, **kw)
 
     def compressor_wave(self, received, finished, handed, wave_blocks):
         """the compressor's next wave (a, b, final), or None (ZopfliB200CompressorWave); finished: 0 or False while
@@ -548,6 +558,20 @@ class Library:
                                                  C.byref(f)):
             return None
         return a.value, b.value, bool(f.value)
+
+    def compressor_wave_units(self, received, finished, handed, wave_blocks, floor=0, dict_len=0, interval=0):
+        """the compressor's next wave as units (ZopfliB200CompressorWaveUnits): ([(a, b, floor, restart), ...],
+        final), or None when no wave is ready"""
+        n = self.lib.ZopfliB200CompressorWaveUnits(received, int(finished), handed, floor, dict_len, interval,
+                                                   wave_blocks, None, None, None, None, 0, None)
+        if n == 0:
+            return None
+        a, b, fl = (np.zeros(n, np.uint64) for _ in range(3))
+        r, f = np.zeros(n, np.int32), C.c_int(0)
+        self.lib.ZopfliB200CompressorWaveUnits(received, int(finished), handed, floor, dict_len, interval, wave_blocks,
+                                               a.ctypes.data, b.ctypes.data, fl.ctypes.data, r.ctypes.data, n,
+                                               C.byref(f))
+        return [(int(a[i]), int(b[i]), int(fl[i]), bool(r[i])) for i in range(n)], bool(f.value)
 
     def splice_spans(self, spans, prefix=b"", bp0=0) -> tuple[bytes, int]:
         """appends spans behind `prefix`, whose last byte has bp0 bits in use -> (bytes, final bp)"""
@@ -629,10 +653,13 @@ class Compressor:
     """ZopfliB200Compressor: input in pieces, ZopfliCompress's bytes out (include/zopfli_b200.h, "input in
     pieces").  Use it as a context manager, or close() it; closing an unfinished compressor abandons it."""
 
-    def __init__(self, lib, fmt=ZOPFLI_FORMAT_GZIP, device=None, stream=None, zdict=None, **kw):
+    def __init__(self, lib, fmt=ZOPFLI_FORMAT_GZIP, device=None, stream=None, zdict=None, restart_interval=None,
+                 **kw):
         self._c = None
         if zdict is not None and fmt == ZOPFLI_FORMAT_GZIP:
             raise ValueError("gzip has no field for a preset dictionary")
+        if restart_interval is not None and restart_interval < 1:
+            raise ValueError("a restart interval is at least one byte")
         self._lib, self._stream = lib, None
         dev = -1
         if device is not None:
@@ -654,12 +681,14 @@ class Compressor:
                                            C.byref(handle)) != 0:
             raise ValueError("ZopfliB200CompressorNew: unknown format, or no such device")
         self._c = handle
-        if zdict is not None:
-            try:
+        try:
+            if zdict is not None:
                 self._set_dictionary(zdict)
-            except BaseException:
-                self.close()
-                raise
+            if restart_interval is not None and lib.lib.ZopfliB200CompressorSetRestartInterval(handle, restart_interval):
+                raise ValueError("ZopfliB200CompressorSetRestartInterval refused the interval")
+        except BaseException:
+            self.close()
+            raise
 
     def _set_dictionary(self, zdict):
         if self._dev >= 0:
@@ -717,6 +746,17 @@ class Compressor:
             return b""
         raise ValueError("unsupported flush mode %r: Z_NO_FLUSH, Z_SYNC_FLUSH, Z_FULL_FLUSH or Z_FINISH" % (mode,))
 
+    def restart_points(self) -> list:
+        """[(data_off, stream_off), ...]: one entry per full flush, automatic or explicit, whose marker has been
+        returned.  stream_off counts from the first byte returned, header included, and
+        zlib.decompressobj(-15).decompress(stream[stream_off:]) starts with data[data_off:]."""
+        if self._c is None:
+            raise ValueError("compressor is closed")
+        n = self._lib.lib.ZopfliB200CompressorRestartPoints(self._c, None, None, 0)
+        d, s = np.zeros(max(n, 1), np.uint64), np.zeros(max(n, 1), np.uint64)
+        n = self._lib.lib.ZopfliB200CompressorRestartPoints(self._c, d.ctypes.data, s.ctypes.data, n)
+        return [(int(d[i]), int(s[i])) for i in range(n)]
+
     def close(self):
         if self._c is not None:
             self._lib.lib.ZopfliB200CompressorFree(self._c)
@@ -746,6 +786,7 @@ def compress(data: bytes, fmt: int = ZOPFLI_FORMAT_GZIP, **options) -> bytes:
     return library().compress(data, fmt, **options)
 
 
-def compressobj(fmt: int = ZOPFLI_FORMAT_GZIP, device=None, stream=None, zdict=None, **options) -> Compressor:
+def compressobj(fmt: int = ZOPFLI_FORMAT_GZIP, device=None, stream=None, zdict=None, restart_interval=None,
+                **options) -> Compressor:
     """a compressor fed in pieces (Library.compressobj), like zlib.compressobj"""
-    return library().compressobj(fmt, device, stream, zdict, **options)
+    return library().compressobj(fmt, device, stream, zdict, restart_interval, **options)

@@ -118,12 +118,30 @@ void seam_plan_out(const BlockPlan& b, Piece& p, unsigned char* len320, uint64_t
   p.tree_bits = b.tree_bits;
 }
 
-void deflate_span_records(Engine& eng, const ZopfliOptions* opt, size_t base, size_t start, size_t end, bool final,
-                          const std::function<void(size_t, size_t, unsigned char*)>& read, SpanRecords& out) {
+void deflate_span_records(Engine& eng, const ZopfliOptions* opt, size_t base, const std::vector<Unit>& units,
+                          bool final, const std::function<void(size_t, size_t, unsigned char*)>& read,
+                          SpanRecords& out) {
+  std::vector<Piece> unit_pieces;
+  deflate_units(eng, opt, 2, final, units, base, unit_pieces);
+  // The marker after every unit that ends at a restart point: an empty stored piece (ZopfliDeflatePart with
+  // btype 0 over an empty range).  It keeps the unit index of the piece before it, so that layout_pieces counts
+  // no unit start for it: markers belong to no unit.
   std::vector<Piece>& pieces = out.pieces;
   pieces.clear();
   out.recs.clear();
-  deflate_units(eng, opt, 2, final, master_blocks(start, end), base, pieces);
+  out.markers.clear();
+  for (size_t i = 0; i < unit_pieces.size(); i++) {
+    pieces.push_back(unit_pieces[i]);
+    const Unit& u = units[unit_pieces[i].unit];
+    if (u.restart && (i + 1 == unit_pieces.size() || unit_pieces[i + 1].unit != unit_pieces[i].unit)) {
+      Piece m;
+      m.type = 0;
+      m.unit = unit_pieces[i].unit;
+      m.instart = m.inend = u.b;
+      out.markers.push_back(pieces.size());
+      pieces.push_back(m);
+    }
+  }
   // Records: maximal runs of compressed pieces, each emitted on the device from bit offset 0 of a
   // byte-aligned slot of one download buffer, and stored pieces as raw bytes.
   std::vector<std::pair<size_t, uint64_t>> runs;    // (record, first bit in the download buffer)
@@ -330,6 +348,8 @@ int (*g_pointer_device)(const void*) = nullptr;
 // Positions are counted in X = preset dictionary || data.  A flush ends a segment: what is left becomes one
 // wave however short, the sync marker follows it, and the next segment's master blocks count from there.  A
 // full flush also raises the floor, the first position a later parse may see: the next slot starts there.
+// Restart points (an interval N) end segments inside the waves instead: each unit carries its floor, and the
+// full-flush marker after a unit that ends at a restart point is one more record of its wave.
 struct ZopfliB200Compressor {
   struct Run {
     Wave w;
@@ -348,7 +368,8 @@ struct ZopfliB200Compressor {
   size_t wave_blocks = 0;            // master blocks per wave, set when the first byte arrives
   size_t received = 0, handed = 0;   // positions: end of the bytes written; end of the bytes in waves
   size_t dict_len = 0;               // position of the first data byte
-  size_t floor = 0;                  // position of the last full flush
+  size_t floor = 0;                  // position of the last full flush at or before `handed`
+  size_t interval = 0;               // restart interval (0: none): automatic full flushes at dict_len + k * interval
   bool started = false;              // a Write or Flush was accepted: no dictionary any more
   bool has_dict = false;
   uint32_t dictid = 0;               // Adler-32 of the whole dictionary
@@ -362,10 +383,14 @@ struct ZopfliB200Compressor {
   size_t pendsize = 0;
   unsigned char bp = 0;
   bool header_done = false;
+  size_t header_bytes = 0;           // bytes of the container header
   uint64_t deflate_bits = 0;         // bits of the deflate stream spliced so far
   size_t produced = 0;               // bytes returned so far
   uint32_t sum;                      // checksum of the bytes of the spliced waves
   std::vector<uint64_t> layout;      // bit offset of every master block spliced so far
+  // (data_off, stream_off) of every full-flush marker spliced so far: data position of the flush, and stream
+  // offset of the first byte after the marker
+  std::vector<std::pair<uint64_t, uint64_t>> index;
   double busy_ms = 0;                // time spent in Write and Finish
 
   ZopfliB200Compressor(const ZopfliOptions* o, ZopfliFormat f, WaveStaging* st)
@@ -411,15 +436,15 @@ struct ZopfliB200Compressor {
       if (staging->device() < 0) ck = std::thread([&] { r.sum = staging->checksum(*eng, r.slot, off, n, kind); });  // overlaps the GPU work
       else r.sum = staging->checksum(*eng, r.slot, off, n, kind);
     }
-    deflate_span_records(*eng, &opt, r.base, r.w.a, r.w.b, r.w.final,
+    deflate_span_records(*eng, &opt, r.base, r.w.units, r.w.final,
                          [&](size_t pos, size_t len, unsigned char* dst) { staging->read(*eng, r.slot, pos - r.base, len, dst); },
                          r.sr);
     if (ck.joinable()) ck.join();
     r.done = true;
   }
 
-  // starts wave w on the filling slot; a wave that is not the last hands its last 32 KiB above the floor to a
-  // fresh slot
+  // starts wave w on the filling slot; a wave that is not the last hands its last 32 KiB above the floor at its
+  // end (w.floor_end) to a fresh slot
   void launch(const Wave& w) {
     while (inflight.size() >= max_inflight()) retire_oldest();
     if (fill < 0) take_slot(floor);  // an empty stream
@@ -431,6 +456,7 @@ struct ZopfliB200Compressor {
     p->worker = std::thread([this, p] { compress(*p); });
     inflight.push_back(std::move(r));
     handed = w.b;
+    floor = w.floor_end;
     fill = -1;
     if (w.final) return;
     const size_t base = wave_base(w.b, floor);
@@ -441,7 +467,8 @@ struct ZopfliB200Compressor {
   void put_header() {
     if (header_done) return;
     unsigned char hdr[10];
-    append_bytes(hdr, container_header(fmt, hdr, has_dict ? &dictid : nullptr), &pend, &pendsize);
+    header_bytes = (size_t)container_header(fmt, hdr, has_dict ? &dictid : nullptr);
+    append_bytes(hdr, header_bytes, &pend, &pendsize);
     header_done = true;
   }
 
@@ -456,6 +483,11 @@ struct ZopfliB200Compressor {
     std::vector<uint64_t> ub;
     const uint64_t end = place_pieces(r->sr.pieces, r->base, phase, ep, &ub, opt.verbose != 0);
     for (size_t i = 0; i + 1 < ub.size(); i++) layout.push_back(deflate_bits + ub[i]);
+    // deflate_bits - phase is the body bit of the wave's bit 0, a byte boundary; after a marker the stream is
+    // byte-aligned
+    for (size_t m : r->sr.markers)
+      index.push_back({r->sr.pieces[m].instart - dict_len,
+                       header_bytes + (deflate_bits - phase + stored_end(ep[m].bit_start, 0)) / 8});
     deflate_bits += end - phase;
     splice_pieces(r->sr.recs, r->sr.stored.data(), &bp, &pend, &pendsize);
     const uint64_t n = r->w.b - r->w.a;
@@ -494,15 +526,53 @@ struct ZopfliB200Compressor {
     return 0;
   }
 
+  // the sync marker behind everything spliced so far; a full one (mode 3) raises the floor to the bytes
+  // received and enters the index.  The stream is then byte-aligned.
+  void put_marker(bool full) {
+    while (!inflight.empty()) retire_oldest();
+    put_header();
+    SpanPiece marker;
+    marker.stored = true;
+    marker.final = false;
+    marker.instart = marker.inend = 0;
+    splice_pieces({marker}, nullptr, &bp, &pend, &pendsize);
+    deflate_bits = stored_end(deflate_bits, 0);
+    if (!full) return;
+    floor = received;
+    if (fill >= 0) fill_base = floor;  // the filling slot holds nothing past the floor: drop what it carried
+    index.push_back({received - dict_len, header_bytes + deflate_bits / 8});
+  }
+
+  int set_restart_interval(size_t n) {
+    if (n == 0 || interval != 0 || started || finished) return 1;
+    interval = n;
+    return 0;
+  }
+
+  // entries of the index whose marker's bytes have been returned
+  size_t restart_points(uint64_t* data_off, uint64_t* stream_off, size_t cap) const {
+    size_t k = 0;
+    while (k < index.size() && index[k].second <= produced) k++;
+    for (size_t i = 0; i < k && i < cap; i++) {
+      if (data_off) data_off[i] = index[i].first;
+      if (stream_off) stream_off[i] = index[i].second;
+    }
+    return k;
+  }
+
   int write(const unsigned char* chunk, size_t n, unsigned char** out, size_t* outsize) {
     if (!out || !outsize || finished || !staging->accepts(chunk, n)) return 1;
     const double t0 = now_ms();
     started = true;
     if (n) {
       set_wave_blocks();
+      // A flush that ended exactly at a restart point: its automatic full flush comes now that a byte past the
+      // point arrives.  (A wave ends at a restart point only with a byte past it, and then carries the marker.)
+      if (handed == received && received > dict_len && interval && (received - dict_len) % interval == 0)
+        put_marker(true);
       const size_t at = received, total = received + n;
       Wave w;
-      while (next_wave(total, false, handed, wave_blocks, &w)) {
+      while (next_wave(total, kWaveWrite, handed, floor, dict_len, interval, wave_blocks, &w)) {
         fill_to(w.b, chunk, at);
         launch(w);
       }
@@ -521,22 +591,11 @@ struct ZopfliB200Compressor {
     const double t0 = now_ms();
     started = true;
     Wave w;
-    const bool full = mode == 3;
-    if (next_wave(received, kWaveFlush, handed, wave_blocks, &w)) {
-      if (full) floor = w.b;  // before launch: the next slot starts at the floor, with nothing carried
+    if (next_wave(received, kWaveFlush, handed, floor, dict_len, interval, wave_blocks, &w)) {
+      if (mode == 3) w.floor_end = w.b;  // the next slot starts at the floor, with nothing carried
       launch(w);
-    } else if (full) {
-      floor = received;
-      if (fill >= 0) fill_base = floor;  // the filling slot holds nothing past the floor: drop what it carried
     }
-    while (!inflight.empty()) retire_oldest();
-    put_header();
-    SpanPiece marker;
-    marker.stored = true;
-    marker.final = false;
-    marker.instart = marker.inend = 0;
-    splice_pieces({marker}, nullptr, &bp, &pend, &pendsize);
-    deflate_bits = stored_end(deflate_bits, 0);
+    put_marker(mode == 3);
     hand_out(out, outsize, true);
     busy_ms += now_ms() - t0;
     return 0;
@@ -547,7 +606,7 @@ struct ZopfliB200Compressor {
     const double t0 = now_ms();
     finished = true;
     Wave w;
-    next_wave(received, kWaveFinish, handed, wave_blocks, &w);
+    next_wave(received, kWaveFinish, handed, floor, dict_len, interval, wave_blocks, &w);
     launch(w);
     while (!inflight.empty()) retire_oldest();
     const size_t insize = received - dict_len;
@@ -607,7 +666,7 @@ void ZopfliDeflatePart(const ZopfliOptions* options, int btype, int final, const
   std::vector<Piece> pieces;
   Engine::Lease eng;
   eng->set_input_host(in + base, inend - base);
-  deflate_units(*eng, options, btype, final != 0, {{instart, inend}}, base, pieces);
+  deflate_units(*eng, options, btype, final != 0, {Unit{instart, inend}}, base, pieces);
   assemble(*eng, pieces, base, bp, out, outsize, nullptr, options->verbose != 0);
 }
 
@@ -639,7 +698,7 @@ int ZopfliB200DeflateSpan(const ZopfliOptions* options, const unsigned char* in,
     eng->set_input_host(in + base, end - base);
   }
   SpanRecords sr;
-  deflate_span_records(*eng, options, base, start, end, final != 0,
+  deflate_span_records(*eng, options, base, master_blocks(start, end), final != 0,
                        [&](size_t pos, size_t n, unsigned char* dst) { memcpy(dst, in + pos, n); }, sr);
   size_t total = 0;
   for (const SpanPiece& r : sr.recs) total += 10 + (r.stored ? r.inend - r.instart : r.bits.bytes.size());
@@ -731,17 +790,41 @@ int ZopfliB200CompressorSetDictionary(ZopfliB200Compressor* c, const unsigned ch
   return c ? c->set_dictionary(dict, n) : 1;
 }
 
+int ZopfliB200CompressorSetRestartInterval(ZopfliB200Compressor* c, size_t interval) {
+  return c ? c->set_restart_interval(interval) : 1;
+}
+
+size_t ZopfliB200CompressorRestartPoints(ZopfliB200Compressor* c, uint64_t* data_off, uint64_t* stream_off, size_t cap) {
+  return c ? c->restart_points(data_off, stream_off, cap) : 0;
+}
+
 void ZopfliB200CompressorFree(ZopfliB200Compressor* c) { delete c; }
 
 int ZopfliB200CompressorWave(size_t received, int finished, size_t handed, size_t wave_blocks, size_t* a, size_t* b,
                              int* final) {
   Wave w;
   const int call = finished == kWaveFlush ? (int)kWaveFlush : (finished != 0 ? (int)kWaveFinish : (int)kWaveWrite);
-  if (!next_wave(received, call, handed, wave_blocks, &w)) return 0;
+  if (!next_wave(received, call, handed, 0, 0, 0, wave_blocks, &w)) return 0;
   *a = w.a;
   *b = w.b;
   *final = w.final ? 1 : 0;
   return 1;
+}
+
+size_t ZopfliB200CompressorWaveUnits(size_t received, int finished, size_t handed, size_t floor, size_t dict_len,
+                                     size_t interval, size_t wave_blocks, size_t* a, size_t* b, size_t* floors,
+                                     int* restart, size_t cap, int* final) {
+  Wave w;
+  const int call = finished == kWaveFlush ? (int)kWaveFlush : (finished != 0 ? (int)kWaveFinish : (int)kWaveWrite);
+  if (!next_wave(received, call, handed, floor, dict_len, interval, wave_blocks, &w)) return 0;
+  for (size_t i = 0; i < w.units.size() && i < cap; i++) {
+    if (a) a[i] = w.units[i].a;
+    if (b) b[i] = w.units[i].b;
+    if (floors) floors[i] = w.units[i].floor;
+    if (restart) restart[i] = w.units[i].restart ? 1 : 0;
+  }
+  if (final) *final = w.final ? 1 : 0;
+  return w.units.size();
 }
 
 size_t ZopfliB200LastMasterBitOffsets(uint64_t* offsets, size_t cap) {

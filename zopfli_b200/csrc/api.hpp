@@ -14,13 +14,16 @@ namespace zb {
 struct BlockPlan;
 struct Piece;
 struct SpanRecords;
+struct Unit;
 class Engine;
 
-// ZopfliB200DeflateSpan's body: master blocks [start, end) of the input, whose bytes from position `base` on
-// the engine already holds, as span records.  read(pos, n, dst) copies input bytes [pos, pos + n) to the host:
+// ZopfliB200DeflateSpan's body: the units of the input (master blocks, each with its floor), whose bytes from
+// position `base` on the engine already holds, as span records; after every unit marked `restart` comes a sync
+// marker (an empty stored block of BFINAL 0).  read(pos, n, dst) copies input bytes [pos, pos + n) to the host:
 // the payloads of stored blocks.
-void deflate_span_records(Engine& eng, const ZopfliOptions* opt, size_t base, size_t start, size_t end, bool final,
-                          const std::function<void(size_t, size_t, unsigned char*)>& read, SpanRecords& out);
+void deflate_span_records(Engine& eng, const ZopfliOptions* opt, size_t base, const std::vector<Unit>& units,
+                          bool final, const std::function<void(size_t, size_t, unsigned char*)>& read,
+                          SpanRecords& out);
 
 // Where a compressor (ZopfliB200Compressor) keeps the bytes of its waves: host memory here, device memory in
 // device_api.cpp.  Slot s holds stream bytes from the slot's base on; it grows as bytes are put into it.

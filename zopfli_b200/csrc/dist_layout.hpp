@@ -5,6 +5,7 @@
 #include <stddef.h>
 #include <stdint.h>
 
+#include <algorithm>
 #include <utility>
 #include <vector>
 
@@ -16,39 +17,76 @@ inline size_t dist_num_master_blocks(size_t insize) {  // deflate.c:912-924 do/w
   return insize == 0 ? 1 : (insize + kMasterBlock - 1) / kMasterBlock;
 }
 
+// A unit of the driver (deflate_units): a master block, or the single range of a ZopfliDeflatePart call.  Its
+// bytes [a, b) are parsed seeing no byte before `floor` (squeeze.c:229-230 on the input from floor on).  In a
+// compressor's wave, `restart` marks a unit that ends at a restart point: the full-flush marker follows it.
+struct Unit {
+  size_t a, b;
+  size_t floor = 0;
+  bool restart = false;
+};
+
 // The master blocks of bytes [a, b) (deflate.c:912-924): kMasterBlock bytes each from a, the last one
 // shorter.  The do/while makes an empty range one empty master block.
-inline std::vector<std::pair<size_t, size_t>> master_blocks(size_t a, size_t b) {
-  std::vector<std::pair<size_t, size_t>> u;
+inline std::vector<Unit> master_blocks(size_t a, size_t b) {
+  std::vector<Unit> u;
   do {
     u.push_back({a, b - a > (size_t)kMasterBlock ? a + kMasterBlock : b});
-    a = u.back().second;
+    a = u.back().b;
   } while (a < b);
   return u;
 }
 
+// The first restart point past position p of a compressor with restart interval `interval` (0: none) whose
+// data starts at position d: the points are d + k * interval, k >= 1.  SIZE_MAX when there is none.
+inline size_t next_restart(size_t p, size_t d, size_t interval) {
+  if (interval == 0) return SIZE_MAX;
+  const size_t k = p < d ? 1 : (p - d) / interval + 1;
+  size_t r;
+  if (__builtin_mul_overflow(k, interval, &r) || __builtin_add_overflow(r, d, &r)) return SIZE_MAX;
+  return r;
+}
+
 // The next wave of a compressor fed in pieces (ZopfliB200Compressor): `received` bytes have arrived,
-// `handed` of them already belong to waves, and a wave is `wave_blocks` master blocks.  A wave is whole
-// master blocks counted from the start of its segment (the stream's first byte, or the last flush point).
-// Before Finish a wave is released only once a byte past it has arrived, because its last master block's
-// BFINAL depends on whether more input follows; at Finish (finished == 1) everything left is one final wave
-// (an empty stream or segment: one empty final wave).  At a flush (finished == 2) everything left is one
-// wave that is not final, or none when nothing is left.  Returns false when no wave is ready.  After a final
-// wave there is none.
-struct Wave { size_t a, b; bool final; };
+// `handed` of them already belong to waves, no byte before `floor` may be seen at `handed`, and restart points
+// lie at d + k * interval (next_restart).  Segments are cut at flush points (every wave ends at one) and at
+// restart points; units are the master blocks of segments, counted from the segment's start, so from `handed`
+// and from every restart point inside the wave.  A unit that ends at a restart point before `received` carries
+// `restart`: the automatic full flush there is due once a byte past it has arrived.  The units after it have
+// that point as their floor, and floor_end is the floor at b.
+// While writing (kWaveWrite) a wave is the next wave_blocks whole units, released only once a byte past them
+// has arrived, because the last unit's BFINAL depends on whether more input follows.  At Finish (kWaveFinish)
+// everything left is one final wave (an empty stream or segment: one empty unit).  At a flush (kWaveFlush)
+// everything left is one wave that is not final, or none when nothing is left.  Returns false when no wave is
+// ready.  After a final wave there is none.
+struct Wave {
+  size_t a, b;
+  bool final;
+  size_t floor_end;
+  std::vector<Unit> units;
+};
 enum WaveCall { kWaveWrite = 0, kWaveFinish = 1, kWaveFlush = 2 };
-inline bool next_wave(size_t received, int finished, size_t handed, size_t wave_blocks, Wave* w) {
-  if (finished == kWaveFlush) {
-    *w = {handed, received, false};
-    return received > handed;
-  }
-  if (finished) {
-    *w = {handed, received, true};
-    return true;
-  }
-  const size_t end = handed + (wave_blocks < 1 ? 1 : wave_blocks) * (size_t)kMasterBlock;
-  if (received <= end) return false;
-  *w = {handed, end, false};
+inline bool next_wave(size_t received, int call, size_t handed, size_t floor, size_t d, size_t interval,
+                      size_t wave_blocks, Wave* w) {
+  if (call == kWaveFlush && received <= handed) return false;
+  const size_t nb = wave_blocks < 1 ? 1 : wave_blocks;
+  std::vector<Unit> u;
+  size_t p = handed;
+  do {
+    const size_t r = next_restart(p, d, interval);
+    size_t e = std::min(p + (size_t)kMasterBlock, r);
+    if (call == kWaveWrite && e >= received) return false;
+    e = std::min(e, received);
+    const bool restart = e == r && r < received;
+    u.push_back({p, e, floor, restart});
+    if (restart) floor = e;
+    p = e;
+  } while (call == kWaveWrite ? u.size() < nb : p < received);
+  w->a = handed;
+  w->b = p;
+  w->final = call == kWaveFinish;
+  w->floor_end = floor;
+  w->units.swap(u);
   return true;
 }
 

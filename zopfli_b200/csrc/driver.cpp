@@ -95,6 +95,7 @@ namespace {
 // What the stages learn of one master block: A-B its cuts, C the size of every block's parse, D-E its pieces.
 struct Master {
   size_t ms, me;                       // byte range
+  size_t floor;                        // the unit's floor: no parse of the master block sees a byte before it
   std::vector<size_t> cuts;            // block boundaries in bytes (ms, ..., me): the first split, or the second if it wins
   std::vector<uint32_t> bsize;         // symbols of every first-split block's optimal parse
   std::vector<Piece> pieces;
@@ -173,13 +174,19 @@ Piece choose_block_type(const FinalBlock& fb, const FixedParse* fx) {
   return p;
 }
 
+// The engine's parse range of input bytes [a, b) whose unit has floor `floor` (absolute positions; the engine
+// holds the bytes from in_base on, so a floor below in_base is no floor for it)
+ParseRange parse_range(size_t a, size_t b, size_t in_base, size_t floor, int mode, int numiterations) {
+  return {a - in_base, b - in_base, mode, numiterations, floor > in_base ? floor - in_base : 0};
+}
+
 // btype 0 (deflate.c:826-828): every unit one stored piece
-void deflate_stored(const std::vector<std::pair<size_t, size_t>>& units, bool final_last, std::vector<Piece>& pieces) {
+void deflate_stored(const std::vector<Unit>& units, bool final_last, std::vector<Piece>& pieces) {
   for (size_t m = 0; m < units.size(); m++) {
     Piece p;
     p.type = 0;
-    p.instart = units[m].first;
-    p.inend = units[m].second;
+    p.instart = units[m].a;
+    p.inend = units[m].b;
     p.final = final_last && m + 1 == units.size();
     p.unit = (uint32_t)m;
     pieces.push_back(p);
@@ -187,11 +194,11 @@ void deflate_stored(const std::vector<std::pair<size_t, size_t>>& units, bool fi
 }
 
 // btype 1 (deflate.c:829-841): one fixed-tree optimal parse per unit
-void deflate_fixed(Engine& eng, const std::vector<std::pair<size_t, size_t>>& units, size_t in_base, bool final_last,
+void deflate_fixed(Engine& eng, const std::vector<Unit>& units, size_t in_base, bool final_last,
                    std::vector<Piece>& pieces) {
   const size_t nm = units.size();
   std::vector<ParseRange> pr;
-  for (auto& u : units) pr.push_back({u.first - in_base, u.second - in_base, 2, 0});
+  for (const Unit& u : units) pr.push_back(parse_range(u.a, u.b, in_base, u.floor, 2, 0));
   std::vector<uint32_t> sizes;
   std::vector<uint64_t> costs;
   eng.parse_keep(pr, Engine::kFix, sizes, costs, 0);
@@ -207,8 +214,8 @@ void deflate_fixed(Engine& eng, const std::vector<std::pair<size_t, size_t>>& un
     p.off = pr[m].instart;
     p.n = sizes[m];
     p.nbits = pc[m].fixed;
-    p.instart = units[m].first;
-    p.inend = units[m].second;
+    p.instart = units[m].a;
+    p.inend = units[m].b;
     p.final = final_last && m + 1 == nm;
     p.unit = (uint32_t)m;
     pieces.push_back(p);
@@ -270,7 +277,7 @@ struct Call {
     // never leave the device: they become the stores of the split service, and only the byte positions
     // of the chosen split points come back (blocksplitter.c:303-313)
     std::vector<ParseRange> pr;
-    for (size_t m : cm) pr.push_back({M[m].ms - in_base, M[m].me - in_base, 0, 0});
+    for (size_t m : cm) pr.push_back(parse_range(M[m].ms, M[m].me, in_base, M[m].floor, 0, 0));
     std::vector<uint32_t> gsize;
     eng.greedy_to_split(pr, gsize, lane);
     const double t1 = now_ms();
@@ -305,7 +312,7 @@ struct Call {
     std::vector<ParseRange> pr;
     for (const BlockRef& k : blocks) {
       const std::vector<size_t>& cuts = M[k.first].cuts;
-      pr.push_back({cuts[k.second] - in_base, cuts[k.second + 1] - in_base, 1, opt->numiterations});
+      pr.push_back(parse_range(cuts[k.second], cuts[k.second + 1], in_base, M[k.first].floor, 1, opt->numiterations));
     }
     const bool want_iters = opt->verbose || opt->verbose_more;
     std::vector<uint32_t> sizes;
@@ -428,7 +435,7 @@ struct Call {
         FinalBlock fb{M[ms[q]].cuts[i], M[ms[q]].cuts[i + 1], j.off + ls, (uint32_t)(le - ls), j.cost[i], j.plan[i]};
         if (le > ls && (j.total < 1000 || (double)fb.c.fixed <= (double)fb.c.dyn * 1.1)) {  // deflate.c:760
           fb.fixed_req = (int)prf.size();
-          prf.push_back({fb.a - in_base, fb.b - in_base, 2, 0});
+          prf.push_back(parse_range(fb.a, fb.b, in_base, M[ms[q]].floor, 2, 0));
         }
         finals[q].push_back(fb);
       }
@@ -534,9 +541,8 @@ struct Call {
 
 }  // namespace
 
-void deflate_units(Engine& eng, const ZopfliOptions* opt, int btype, bool final_last,
-                   const std::vector<std::pair<size_t, size_t>>& units, size_t in_base,
-                   std::vector<Piece>& pieces) {
+void deflate_units(Engine& eng, const ZopfliOptions* opt, int btype, bool final_last, const std::vector<Unit>& units,
+                   size_t in_base, std::vector<Piece>& pieces) {
   if (btype == 0) {
     deflate_stored(units, final_last, pieces);
     return;
@@ -552,7 +558,11 @@ void deflate_units(Engine& eng, const ZopfliOptions* opt, int btype, bool final_
   const size_t nm = units.size();
   const Schedule s = schedule(nm, eng.device_memory_total());
   Call call{eng, opt, in_base, final_last, s.giant, std::vector<Master>(nm)};
-  for (size_t m = 0; m < nm; m++) { call.M[m].ms = units[m].first; call.M[m].me = units[m].second; }
+  for (size_t m = 0; m < nm; m++) {
+    call.M[m].ms = units[m].a;
+    call.M[m].me = units[m].b;
+    call.M[m].floor = units[m].floor;
+  }
   std::vector<std::vector<size_t>> chunks(s.nchunks);
   for (size_t m = 0; m < nm; m++) chunks[m * s.nchunks / nm].push_back(m);
   std::vector<std::thread> th;

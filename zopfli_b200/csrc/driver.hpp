@@ -10,6 +10,7 @@
 #include <vector>
 
 #include "../../include/zopfli.h"
+#include "dist_layout.hpp"
 #include "engine.hpp"
 
 namespace zb {
@@ -43,12 +44,14 @@ struct SpanPiece {
   bool final = false;
 };
 
-// ZopfliB200DeflateSpan's records of a range of master blocks: the driver's pieces, and the records made
-// of them (maximal runs of compressed pieces as bits, stored pieces as ranges of `stored`, their bytes).
+// ZopfliB200DeflateSpan's records of a range of units: the driver's pieces, and the records made of them
+// (maximal runs of compressed pieces as bits, stored pieces as ranges of `stored`, their bytes).  `markers`
+// indexes the pieces that are full-flush markers after units that end at a restart point.
 struct SpanRecords {
   std::vector<Piece> pieces;
   std::vector<SpanPiece> recs;
   std::vector<unsigned char> stored;
+  std::vector<size_t> markers;
 };
 
 struct HostTimes { double split = 0, emit = 0, other = 0; };
@@ -84,11 +87,11 @@ void parallel_for(size_t n, F fn) {
   for (auto& t : th) t.join();
 }
 
-// Compresses the given byte ranges ("units": master blocks, or the single range of a
-// ZopfliDeflatePart call) of the input; the engine must already hold its bytes [in_base ...).
-void deflate_units(Engine& eng, const ZopfliOptions* opt, int btype, bool final_last,
-                   const std::vector<std::pair<size_t, size_t>>& units, size_t in_base,
-                   std::vector<Piece>& pieces);
+// Compresses the given units of the input (dist_layout.hpp Unit: master blocks, or the single range of a
+// ZopfliDeflatePart call, each with its floor); the engine must already hold its bytes [in_base ...).  Every
+// parse of a unit sees no byte before the unit's floor.
+void deflate_units(Engine& eng, const ZopfliOptions* opt, int btype, bool final_last, const std::vector<Unit>& units,
+                   size_t in_base, std::vector<Piece>& pieces);
 
 // Master blocks that deflate_units runs at once on a device with this much memory (chunk pipelines x batch,
 // both from its schedule): the wave of a long ZopfliCompress call.  ZopfliB200Compressor asks for half the

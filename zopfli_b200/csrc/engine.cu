@@ -468,14 +468,19 @@ struct Engine::Impl {
       // a range of at most 0x7fff0000 bytes keeps npos and nkeys (range + 32 KiB) in the 32-bit counts of SegDesc,
       // and every position and key index below 2^31 for the kernels' 32-bit index arithmetic (traced-path entries,
       // position << 9 | length, are 64-bit for that reason)
-      if (r[i].inend < r[i].instart || r[i].inend > insize || r[i].inend - r[i].instart > 0x7fff0000ull) {
-        fprintf(stderr, "zopfli-b200: bad parse range [%llu,%llu) for input of %llu bytes\n",
-                (unsigned long long)r[i].instart, (unsigned long long)r[i].inend, (unsigned long long)insize);
+      if (r[i].inend < r[i].instart || r[i].inend > insize || r[i].inend - r[i].instart > 0x7fff0000ull ||
+          r[i].floor > r[i].instart) {
+        fprintf(stderr, "zopfli-b200: bad parse range [%llu,%llu) floor %llu for input of %llu bytes\n",
+                (unsigned long long)r[i].instart, (unsigned long long)r[i].inend, (unsigned long long)r[i].floor,
+                (unsigned long long)insize);
         abort();
       }
       s.instart = r[i].instart;
       s.inend = r[i].inend;
-      s.winstart = s.instart > (uint64_t)kWindow ? s.instart - kWindow : 0;  // squeeze.c:229-230
+      // squeeze.c:229-230 on in + floor: the kernels see the window only through winstart (k_keys hashes
+      // [winstart, inend), k_match's candidates are those keys), so a floor needs no device code of its own
+      s.winstart = s.instart > (uint64_t)kWindow ? s.instart - kWindow : 0;
+      if (s.winstart < r[i].floor) s.winstart = r[i].floor;
       s.key_off = L.nkeys;
       s.pos_off = L.npos;
       s.nkeys = (uint32_t)(s.inend - s.winstart);

@@ -12,6 +12,8 @@ struct ParseRange {
   int mode;           // 0 greedy parse only (ZopfliLZ77Greedy), 1 optimal parse (ZopfliLZ77Optimal),
                       // 2 optimal parse with fixed-tree costs (ZopfliLZ77OptimalFixed)
   int numiterations;  // mode 1 only
+  uint64_t floor = 0; // first byte the parse may see (a compressor's last full flush): the window starts at
+                      // max(instart - 32768, floor), as the reference's parse of in + floor would see it
 };
 
 struct ParseResult {        // symbols of range i: [off[i], off[i]+size[i]) in ll / d
