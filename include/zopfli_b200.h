@@ -283,6 +283,32 @@ size_t ZopfliB200CompressorRestartPoints(ZopfliB200Compressor* c, uint64_t* data
 size_t ZopfliB200CompressorWaveUnits(size_t received, int finished, size_t handed, size_t floor, size_t dict_len,
                                      size_t interval, size_t wave_blocks, size_t* a, size_t* b, size_t* floors,
                                      int* restart, size_t cap, int* final);
+/* Output in device memory: a device compressor (device >= 0) keeps its stream on the device.  Each wave's runs of
+ * compressed blocks are emitted on the device into an allocation of the wave's own, and k_splice places them and
+ * the wave's stored blocks (read from its staging slot) at the stream's bit position in a pending buffer on the
+ * device; the header, the markers and the trailer are written by the same kernel.  So no compressed byte is
+ * downloaded except those a caller asks for on the host.
+ * WriteToDevice, FlushToDevice and FinishToDevice are Write, Flush and Finish with the output in device memory:
+ * the same bytes are complete after each call, so the byte counts per call match, and the calls of both kinds
+ * may be mixed on one compressor (the stream is the concatenation in call order).  *dev_out is exactly *outsize
+ * bytes from cudaMallocAsync on cuda_stream, as ZopfliB200CompressDeviceToDevice's result: outputs only, nothing
+ * appended, the caller frees it (ZopfliB200FreeDevice / cudaFreeAsync); NULL and 0 when the call completes no
+ * byte.  The call returns once the bytes are in place, and cuda_stream waits for them.  They return nonzero,
+ * every output untouched, for everything Write, Flush and Finish refuse and for a host compressor (device < 0).
+ * Write, Flush and Finish on a device compressor download exactly the bytes they return, once.
+ * Device memory of a device compressor: the staging above; plus, for each wave in flight, its runs of compressed
+ * blocks, at most the wave's bytes plus 5 bytes per started 65,535 bytes of each block (no compressed block is
+ * larger than its stored form) plus 8 bytes per run; plus the pending stream of one call, a buffer that grows
+ * by doubling and is kept: at most twice the most bytes one call has returned, plus 4. */
+int ZopfliB200CompressorWriteToDevice(ZopfliB200Compressor* c, const unsigned char* chunk, size_t n,
+                                      unsigned char** dev_out, size_t* outsize);
+int ZopfliB200CompressorFlushToDevice(ZopfliB200Compressor* c, int mode, unsigned char** dev_out, size_t* outsize);
+int ZopfliB200CompressorFinishToDevice(ZopfliB200Compressor* c, unsigned char** dev_out, size_t* outsize);
+/* seam: ZopfliB200AppendSpan with the splice done by k_splice on the current device (product library only): the
+ * span is validated as AppendSpan validates it, uploaded with the partly filled last byte, spliced on the device
+ * and the new bytes downloaded.  Returns 1, output untouched, for what AppendSpan refuses and for *bp > 7. */
+int ZopfliB200DeviceAppendSpan(const unsigned char* span, size_t spansize, unsigned char* bp,
+                               unsigned char** out, size_t* outsize);
 
 /* ---- several GPUs, one stream (SURVEY 8(e)) ----
  * The master blocks of one input (the reference's independent unit, deflate.c:908-931) are sharded

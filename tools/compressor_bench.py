@@ -16,8 +16,13 @@ calls Flush(FULL) at each point, so each point ends a wave of its own; the other
 the segments between points share waves.  Their streams must be byte-identical ("identical_to_explicit"), and
 every index entry of the restart leg must inflate raw to the data from its offset on.
 
+With --device-output, one more leg (device chunks, 64 MiB writes) takes its output in device memory
+(compressobj(..., device_output=True)); its stream must be byte-identical to the device-chunk leg's with host
+output ("identical_to_host_output").  Every record then also carries the leg's h2d_bytes and d2h_bytes
+(ZopfliB200Stats), which show what crossed PCIe.
+
     python tools/compressor_bench.py [--mib 430] [--reps 3] [--numiterations 15] [--flush-every BYTES]
-                                     [--restart-every BYTES]
+                                     [--restart-every BYTES] [--device-output]
 """
 import argparse
 import json
@@ -51,10 +56,10 @@ def run_whole(lib, data, kw):
 
 
 def run_pieces(lib, src, write, kw, device, flush_every=0, mode=zlib.Z_SYNC_FLUSH, restart_interval=None,
-               index=None):
+               index=None, device_output=False):
     out = []
     with lib.compressobj(zb.ZOPFLI_FORMAT_GZIP, device=0 if device else None, restart_interval=restart_interval,
-                         **kw) as c:
+                         device_output=device_output, **kw) as c:
         p = 0
         while p < len(src):
             q = min(p + write, len(src))
@@ -68,7 +73,7 @@ def run_pieces(lib, src, write, kw, device, flush_every=0, mode=zlib.Z_SYNC_FLUS
         out.append(c.flush())
         if index is not None:
             index[:] = c.restart_points()
-    return b"".join(out)
+    return torch.cat(out) if device_output else b"".join(out)
 
 
 def index_inflates(stream, data, index):
@@ -84,6 +89,8 @@ def main():
     ap.add_argument("--flush-every", type=int, default=0, help="bytes of input between sync flushes (0: no flush legs)")
     ap.add_argument("--restart-every", type=int, default=0,
                     help="bytes of input between full flushes, explicit and by restart_interval (0: no restart legs)")
+    ap.add_argument("--device-output", action="store_true",
+                    help="a leg with device chunks and output in device memory, and PCIe bytes in every record")
     args = ap.parse_args()
     kw = {"numiterations": args.numiterations}
     lib = zb.library()
@@ -111,14 +118,21 @@ def main():
                      lambda: run_pieces(lib, host_view, 64 * MIB, kw, False, r, zlib.Z_FULL_FLUSH)))
         legs.append(("compressor host 64 MiB, restart_interval=%d" % r,
                      lambda: run_pieces(lib, host_view, 64 * MIB, kw, False, restart_interval=r, index=index)))
-    want, explicit = None, None
+    if args.device_output:
+        legs.append(("compressor device 64 MiB, device output",
+                     lambda: run_pieces(lib, dev, 64 * MIB, kw, True, device_output=True)))
+    want, explicit, device_host_output = None, None, None
     for rep in range(args.reps):
         for name, fn in legs:
             torch.cuda.synchronize()
+            lib.reset_stats()
             t0 = time.perf_counter()
             got = fn()
             torch.cuda.synchronize()
             ms = (time.perf_counter() - t0) * 1e3
+            st = lib.stats()
+            if isinstance(got, torch.Tensor):  # device output: copied to the host for the checks, after the timing
+                got = bytes(got.cpu().numpy())
             if want is None:
                 want = got
             free, total = torch.cuda.mem_get_info(0)
@@ -135,6 +149,12 @@ def main():
                 rec["inflates"] = zlib.decompress(got, 31) == data
             else:
                 rec["identical"] = got == want
+            if name == "compressor device 64 MiB":
+                device_host_output = got
+            elif "device output" in name:
+                rec["identical_to_host_output"] = got == device_host_output
+            if args.device_output:
+                rec["h2d_bytes"], rec["d2h_bytes"] = st["h2d_bytes"], st["d2h_bytes"]
             rec["device_used_GiB"] = round((total - free) / (1 << 30), 2)
             print(json.dumps(rec), flush=True)
     print(json.dumps({"card": card()}), flush=True)

@@ -226,6 +226,12 @@ class Library:
         L.ZopfliB200CompressorRestartPoints.restype = sz
         L.ZopfliB200CompressorWaveUnits.argtypes = [sz, C.c_int, sz, sz, sz, sz, sz, vp, vp, vp, vp, sz, C.POINTER(C.c_int)]
         L.ZopfliB200CompressorWaveUnits.restype = sz
+        L.ZopfliB200CompressorWriteToDevice.argtypes = [vp, vp, sz, C.POINTER(vp), C.POINTER(sz)]
+        L.ZopfliB200CompressorWriteToDevice.restype = C.c_int
+        L.ZopfliB200CompressorFlushToDevice.argtypes = [vp, C.c_int, C.POINTER(vp), C.POINTER(sz)]
+        L.ZopfliB200CompressorFlushToDevice.restype = C.c_int
+        L.ZopfliB200CompressorFinishToDevice.argtypes = [vp, C.POINTER(vp), C.POINTER(sz)]
+        L.ZopfliB200CompressorFinishToDevice.restype = C.c_int
         # device-resident calls and the device emission seam (csrc/device_api.cpp); a host-only test build of the
         # ABI does not export them
         for name, args, res in (("ZopfliB200CompressDeviceToDevice",
@@ -235,7 +241,9 @@ class Library:
                                 ("ZopfliB200Adler32Device", [vp, sz, vp, C.POINTER(C.c_uint32)], C.c_int),
                                 ("ZopfliB200DeviceEmitBlocks", [vp, sz, vp, vp, sz, sz, vp, vp, vp, vp, C.c_uint, vp, sz, vp, vp,
                                                                 vp], C.c_int),
-                                ("ZopfliB200DeviceProbeParts", [vp, sz, vp, vp, vp, vp], C.c_int)):
+                                ("ZopfliB200DeviceProbeParts", [vp, sz, vp, vp, vp, vp], C.c_int),
+                                ("ZopfliB200DeviceAppendSpan", [vp, sz, C.POINTER(C.c_ubyte), C.POINTER(vp), C.POINTER(sz)],
+                                 C.c_int)):
             f = getattr(L, name, None)
             if f is not None:
                 f.argtypes, f.restype = args, res
@@ -538,7 +546,7 @@ class Library:
 
     # ---- input in pieces (ZopfliB200Compressor) ----
     def compressobj(self, fmt=ZOPFLI_FORMAT_GZIP, device=None, stream=None, zdict=None, restart_interval=None,
-                    **kw) -> "Compressor":
+                    device_output=False, **kw) -> "Compressor":
         """A compressor shaped like zlib.compressobj: compress(chunk) -> bytes, flush(mode) -> bytes.  Without
         zdict and sync / full flushes, all outputs concatenated equal compress(<all chunks>, fmt, **kw).
         device=None: chunks are bytes-like objects; device=<index or torch.device>: chunks are contiguous CUDA
@@ -547,8 +555,10 @@ class Library:
         no dependency).  zdict: a preset dictionary (zlib and raw deflate only), bytes-like, or for a device
         compressor also a contiguous uint8 CUDA tensor of its device.  restart_interval=N: a full flush at every
         N bytes of data that has a byte after it, compressed inside the waves; Compressor.restart_points() is the
-        index of where raw inflating can start."""
-        return Compressor(self, fmt, device, stream, zdict, restart_interval, **kw)
+        index of where raw inflating can start.  device_output=True (device compressors only): compress() and
+        flush() return uint8 CUDA tensors on the compressor's device that own the library's allocation (no copy),
+        empty when no byte is complete; the compressed bytes never cross PCIe."""
+        return Compressor(self, fmt, device, stream, zdict, restart_interval, device_output, **kw)
 
     def compressor_wave(self, received, finished, handed, wave_blocks):
         """the compressor's next wave (a, b, final), or None (ZopfliB200CompressorWave); finished: 0 or False while
@@ -573,8 +583,10 @@ class Library:
                                                C.byref(f))
         return [(int(a[i]), int(b[i]), int(fl[i]), bool(r[i])) for i in range(n)], bool(f.value)
 
-    def splice_spans(self, spans, prefix=b"", bp0=0) -> tuple[bytes, int]:
-        """appends spans behind `prefix`, whose last byte has bp0 bits in use -> (bytes, final bp)"""
+    def splice_spans(self, spans, prefix=b"", bp0=0, device=False) -> tuple[bytes, int]:
+        """appends spans behind `prefix`, whose last byte has bp0 bits in use -> (bytes, final bp); device=True
+        splices on the device (ZopfliB200DeviceAppendSpan: k_splice)"""
+        append = self.lib.ZopfliB200DeviceAppendSpan if device else self.lib.ZopfliB200AppendSpan
         out, n, bp = C.c_void_p(None), C.c_size_t(0), C.c_ubyte(bp0)
         if prefix:
             # seed the zopfli-style buffer with the container header
@@ -589,7 +601,7 @@ class Library:
             n = C.c_size_t(len(hdr))
         for s in spans:
             b = np.frombuffer(s, np.uint8)
-            if self.lib.ZopfliB200AppendSpan(b.ctypes.data, len(b), C.byref(bp), C.byref(out), C.byref(n)) != 0:
+            if append(b.ctypes.data, len(b), C.byref(bp), C.byref(out), C.byref(n)) != 0:
                 raise ValueError("malformed span")
         return self._take(out, n), bp.value
 
@@ -654,8 +666,10 @@ class Compressor:
     pieces").  Use it as a context manager, or close() it; closing an unfinished compressor abandons it."""
 
     def __init__(self, lib, fmt=ZOPFLI_FORMAT_GZIP, device=None, stream=None, zdict=None, restart_interval=None,
-                 **kw):
+                 device_output=False, **kw):
         self._c = None
+        if device_output and device is None:
+            raise ValueError("device_output needs a device compressor (device=)")
         if zdict is not None and fmt == ZOPFLI_FORMAT_GZIP:
             raise ValueError("gzip has no field for a preset dictionary")
         if restart_interval is not None and restart_interval < 1:
@@ -674,7 +688,7 @@ class Compressor:
                 self._stream = stream
             else:
                 self._stream = torch.cuda.ExternalStream(int(stream), device=torch.device("cuda", dev))
-        self._dev, self._own_stream = dev, stream is not None
+        self._dev, self._own_stream, self._device_output = dev, stream is not None, bool(device_output)
         handle = C.c_void_p(None)
         o = lib.options(**kw)
         if lib.lib.ZopfliB200CompressorNew(C.byref(o), fmt, dev, self._stream.cuda_stream if dev >= 0 else None,
@@ -718,31 +732,46 @@ class Compressor:
         return ptr, nbytes
 
     def _call(self, fn, *args):
+        """fn's output: host bytes, or with device_output (fn is the *ToDevice twin) a uint8 CUDA tensor"""
         if self._c is None:
             raise ValueError("compressor is closed")
         out, n = C.c_void_p(None), C.c_size_t(0)
         if fn(self._c, *args, C.byref(out), C.byref(n)) != 0:
             raise ValueError("compressor refused the call: it is finished, or the chunk is the wrong kind of memory")
-        return self._lib._take(out, n)
+        if not self._device_output:
+            return self._lib._take(out, n)
+        import torch
+        dev = torch.device("cuda", self._dev)
+        if not n.value:
+            return torch.empty(0, dtype=torch.uint8, device=dev)
+        buf = DeviceOutBuffer(self._lib.lib, out, n.value, self._stream.cuda_stream)
+        return torch.as_tensor(buf)  # keeps buf alive as long as the tensor lives
 
-    def compress(self, chunk) -> bytes:
-        """the output bytes that are complete after this chunk (possibly none)"""
+    def _fn(self, name):
+        return getattr(self._lib.lib, name + ("ToDevice" if self._device_output else ""))
+
+    def compress(self, chunk):
+        """the output bytes that are complete after this chunk (possibly none): bytes, or a CUDA tensor with
+        device_output"""
         if self._dev >= 0:
             ptr, nbytes = self._chunk(chunk)
-            return self._call(self._lib.lib.ZopfliB200CompressorWrite, C.c_void_p(ptr), nbytes)
+            return self._call(self._fn("ZopfliB200CompressorWrite"), C.c_void_p(ptr), nbytes)
         a = np.frombuffer(memoryview(chunk).cast("B"), np.uint8)
-        return self._call(self._lib.lib.ZopfliB200CompressorWrite, a.ctypes.data if len(a) else None, len(a))
+        return self._call(self._fn("ZopfliB200CompressorWrite"), a.ctypes.data if len(a) else None, len(a))
 
-    def flush(self, mode=zlib.Z_FINISH) -> bytes:
+    def flush(self, mode=zlib.Z_FINISH):
         """zlib's flush modes.  Z_FINISH (the default): the rest of the stream with the trailer; the compressor
         takes no more input.  Z_SYNC_FLUSH: everything written so far, byte-aligned and decodable, ending with an
         empty stored block.  Z_FULL_FLUSH: the same, and no later byte refers to what came before, so inflating
-        can start there.  Z_NO_FLUSH: nothing."""
+        can start there.  Z_NO_FLUSH: nothing.  With device_output the result is a CUDA tensor."""
         if mode == zlib.Z_FINISH:
-            return self._call(self._lib.lib.ZopfliB200CompressorFinish)
+            return self._call(self._fn("ZopfliB200CompressorFinish"))
         if mode in (zlib.Z_SYNC_FLUSH, zlib.Z_FULL_FLUSH):
-            return self._call(self._lib.lib.ZopfliB200CompressorFlush, mode)
+            return self._call(self._fn("ZopfliB200CompressorFlush"), mode)
         if mode == zlib.Z_NO_FLUSH:
+            if self._device_output:
+                import torch
+                return torch.empty(0, dtype=torch.uint8, device=torch.device("cuda", self._dev))
             return b""
         raise ValueError("unsupported flush mode %r: Z_NO_FLUSH, Z_SYNC_FLUSH, Z_FULL_FLUSH or Z_FINISH" % (mode,))
 
@@ -787,6 +816,6 @@ def compress(data: bytes, fmt: int = ZOPFLI_FORMAT_GZIP, **options) -> bytes:
 
 
 def compressobj(fmt: int = ZOPFLI_FORMAT_GZIP, device=None, stream=None, zdict=None, restart_interval=None,
-                **options) -> Compressor:
+                device_output=False, **options) -> Compressor:
     """a compressor fed in pieces (Library.compressobj), like zlib.compressobj"""
-    return library().compressobj(fmt, device, stream, zdict, restart_interval, **options)
+    return library().compressobj(fmt, device, stream, zdict, restart_interval, device_output, **options)

@@ -119,8 +119,7 @@ void seam_plan_out(const BlockPlan& b, Piece& p, unsigned char* len320, uint64_t
 }
 
 void deflate_span_records(Engine& eng, const ZopfliOptions* opt, size_t base, const std::vector<Unit>& units,
-                          bool final, const std::function<void(size_t, size_t, unsigned char*)>& read,
-                          SpanRecords& out) {
+                          bool final, SpanRecords& out) {
   std::vector<Piece> unit_pieces;
   deflate_units(eng, opt, 2, final, units, base, unit_pieces);
   // The marker after every unit that ends at a restart point: an empty stored piece (ZopfliDeflatePart with
@@ -143,10 +142,8 @@ void deflate_span_records(Engine& eng, const ZopfliOptions* opt, size_t base, co
     }
   }
   // Records: maximal runs of compressed pieces, each emitted on the device from bit offset 0 of a
-  // byte-aligned slot of one download buffer, and stored pieces as raw bytes.
-  std::vector<std::pair<size_t, uint64_t>> runs;    // (record, first bit in the download buffer)
-  std::vector<std::pair<size_t, size_t>> stored;    // (record, piece)
-  std::vector<Engine::EmitPiece> ep_all;
+  // byte-aligned slot of one buffer, and stored pieces as raw bytes.
+  out.ep.clear();
   uint64_t pos = 0;
   size_t nstored = 0;
   for (size_t i = 0; i < pieces.size();) {
@@ -157,7 +154,7 @@ void deflate_span_records(Engine& eng, const ZopfliOptions* opt, size_t base, co
       r.instart = nstored;
       nstored += pieces[i].inend - pieces[i].instart;
       r.inend = nstored;
-      stored.push_back({out.recs.size(), i});
+      r.src = pieces[i].instart;
       out.recs.push_back(std::move(r));
       i++;
       continue;
@@ -169,24 +166,66 @@ void deflate_span_records(Engine& eng, const ZopfliOptions* opt, size_t base, co
     const uint64_t e = layout_pieces(run, base, pos, ep, nullptr);
     r.final = pieces[j - 1].final;
     r.bits.nbits = e - pos;
-    runs.push_back({out.recs.size(), pos});
+    r.src = pos;
     out.recs.push_back(std::move(r));
-    ep_all.insert(ep_all.end(), ep.begin(), ep.end());
+    out.ep.insert(out.ep.end(), ep.begin(), ep.end());
     pos = (e + 63) & ~(uint64_t)63;  // the next run starts on a fresh word: no shared bytes between records
     i = j;
   }
-  std::vector<unsigned char> bits((size_t)(pos / 8) + 8, 0);
-  if (pos) eng.emit(ep_all, pos, bits.data());
-  for (const auto& r : runs) {
-    BitString& b = out.recs[r.first].bits;
-    const unsigned char* s = bits.data() + r.second / 8;
-    b.bytes.assign(s, s + (size_t)((b.nbits + 7) / 8));
+  out.run_bits = pos;
+  out.stored.clear();
+}
+
+void span_records_to_host(Engine& eng, SpanRecords& sr, const std::function<void(size_t, size_t, unsigned char*)>& read) {
+  std::vector<unsigned char> bits((size_t)(sr.run_bits / 8) + 8, 0);
+  if (sr.run_bits) eng.emit(sr.ep, sr.run_bits, bits.data());
+  size_t nstored = 0;
+  for (const SpanPiece& r : sr.recs) nstored = r.stored ? r.inend : nstored;
+  sr.stored.resize(nstored);
+  for (SpanPiece& r : sr.recs) {
+    if (!r.stored) {
+      const unsigned char* s = bits.data() + r.src / 8;
+      r.bits.bytes.assign(s, s + (size_t)((r.bits.nbits + 7) / 8));
+    } else if (r.inend > r.instart) {
+      read((size_t)r.src, r.inend - r.instart, sr.stored.data() + r.instart);
+    }
   }
-  out.stored.resize(nstored);
-  for (const auto& s : stored) {
-    const Piece& p = pieces[s.second];
-    if (p.inend > p.instart) read(p.instart, p.inend - p.instart, out.stored.data() + out.recs[s.first].instart);
+}
+
+bool parse_span(const unsigned char* span, size_t spansize, std::vector<SpanPiece>& pieces,
+                std::vector<unsigned char>& rawbytes) {
+  size_t o = 0;
+  // validate the whole span before touching the output: spans arrive over a transport
+  while (o < spansize) {
+    if (spansize - o < 10 || span[o] > 1 || span[o + 1] > 1) return false;
+    uint64_t v;
+    memcpy(&v, span + o + 2, 8);
+    const uint64_t nbytes = span[o] == 1 ? v : (v + 7) / 8;
+    if (nbytes > spansize - o - 10) return false;
+    o += 10 + (size_t)nbytes;
   }
+  o = 0;
+  // first pass: collect stored payloads contiguously so Piece offsets can index one buffer
+  while (o + 10 <= spansize) {
+    uint64_t v;
+    memcpy(&v, span + o + 2, 8);
+    bool stored = span[o] == 1;
+    size_t nbytes = stored ? (size_t)v : (size_t)((v + 7) / 8);
+    SpanPiece p;
+    p.stored = stored;
+    p.final = span[o + 1] != 0;
+    if (stored) {
+      p.instart = rawbytes.size();
+      rawbytes.insert(rawbytes.end(), span + o + 10, span + o + 10 + nbytes);
+      p.inend = rawbytes.size();
+    } else {
+      p.bits.bytes.assign(span + o + 10, span + o + 10 + nbytes);
+      p.bits.nbits = v;
+    }
+    pieces.push_back(std::move(p));
+    o += 10 + nbytes;
+  }
+  return true;
 }
 
 }  // namespace zb
@@ -306,9 +345,14 @@ void make_store(const unsigned short* ll, const unsigned short* dd, size_t n, Lz
   st.finalize();
 }
 
-// A compressor's waves in host memory: one buffer per slot, reserved up to the bytes of one staged wave
+// A compressor's waves in host memory: one buffer per slot, reserved up to the bytes of one staged wave; the
+// stream is spliced on the host (splice_pieces) into a zopfli-style buffer
 struct HostStaging : WaveStaging {
   std::vector<unsigned char> slot[kSlots];
+  unsigned char* pend = nullptr;
+  size_t pendsize = 0;
+  unsigned char bp = 0;
+  ~HostStaging() override { free(pend); }
   int device() const override { return -1; }
   bool accepts(const void* p, size_t n) const override {
     return n == 0 || (p && !(g_pointer_device && g_pointer_device(p) >= 0));
@@ -328,8 +372,28 @@ struct HostStaging : WaveStaging {
   uint32_t checksum(Engine&, int s, size_t off, size_t n, int kind) override {
     return host_checksum(at(s, off), n, kind, 0);
   }
-  void read(Engine&, int s, size_t off, size_t n, unsigned char* dst) override { memcpy(dst, at(s, off), n); }
+  void take_records(Engine& eng, int s, size_t base, SpanRecords& sr) override {
+    span_records_to_host(eng, sr, [&](size_t pos, size_t n, unsigned char* dst) { memcpy(dst, at(s, pos - base), n); });
+  }
+  void drop_records(SpanRecords&) override {}
   uint32_t checksum_of(const unsigned char* p, size_t n, int kind) override { return host_checksum(p, n, kind, 0); }
+
+  unsigned phase() const override { return pendsize ? (bp & 7u) : 0u; }
+  void put_bytes(const unsigned char* p, size_t n) override { append_bytes(p, n, &pend, &pendsize); }
+  void splice(int, size_t, const SpanRecords& sr) override { splice_pieces(sr.recs, sr.stored.data(), &bp, &pend, &pendsize); }
+  // What stays behind is at most the partly filled last byte, in a fresh one-byte buffer: zopfli's capacity rule
+  // derives a buffer's capacity from its size, so a larger buffer must not be kept under a smaller size.
+  size_t hand_out(bool all, bool, unsigned char** out, size_t* outsize) override {
+    const size_t keep = (!all && bp != 0 && pendsize > 0) ? 1 : 0;
+    const unsigned char last = keep ? pend[pendsize - 1] : 0;
+    const size_t n = pendsize - keep;
+    append_bytes(pend, n, out, outsize);
+    free(pend);
+    pend = nullptr;
+    pendsize = 0;
+    if (keep) append_bytes(&last, 1, &pend, &pendsize);
+    return n;
+  }
 };
 
 }  // namespace
@@ -378,10 +442,6 @@ struct ZopfliB200Compressor {
   size_t fill_base = 0;              // position of its byte 0
   std::vector<int> free_slots;
   std::deque<std::unique_ptr<Run>> inflight;
-  // the stream not yet returned: at most the partly filled last byte between calls (zopfli-style buffer)
-  unsigned char* pend = nullptr;
-  size_t pendsize = 0;
-  unsigned char bp = 0;
   bool header_done = false;
   size_t header_bytes = 0;           // bytes of the container header
   uint64_t deflate_bits = 0;         // bits of the deflate stream spliced so far
@@ -398,8 +458,10 @@ struct ZopfliB200Compressor {
     for (int s = WaveStaging::kSlots - 1; s >= 0; s--) free_slots.push_back(s);
   }
   ~ZopfliB200Compressor() {  // abandons unfinished work: waits for the waves in flight, drops their output
-    for (auto& r : inflight) r->worker.join();
-    free(pend);
+    for (auto& r : inflight) {
+      r->worker.join();
+      staging->drop_records(r->sr);
+    }
   }
 
   // With verbose reports a wave starts once the one before it is spliced, so reports do not interleave.
@@ -436,9 +498,8 @@ struct ZopfliB200Compressor {
       if (staging->device() < 0) ck = std::thread([&] { r.sum = staging->checksum(*eng, r.slot, off, n, kind); });  // overlaps the GPU work
       else r.sum = staging->checksum(*eng, r.slot, off, n, kind);
     }
-    deflate_span_records(*eng, &opt, r.base, r.w.units, r.w.final,
-                         [&](size_t pos, size_t len, unsigned char* dst) { staging->read(*eng, r.slot, pos - r.base, len, dst); },
-                         r.sr);
+    deflate_span_records(*eng, &opt, r.base, r.w.units, r.w.final, r.sr);
+    staging->take_records(*eng, r.slot, r.base, r.sr);
     if (ck.joinable()) ck.join();
     r.done = true;
   }
@@ -468,7 +529,7 @@ struct ZopfliB200Compressor {
     if (header_done) return;
     unsigned char hdr[10];
     header_bytes = (size_t)container_header(fmt, hdr, has_dict ? &dictid : nullptr);
-    append_bytes(hdr, header_bytes, &pend, &pendsize);
+    staging->put_bytes(hdr, header_bytes);
     header_done = true;
   }
 
@@ -478,7 +539,7 @@ struct ZopfliB200Compressor {
     inflight.pop_front();
     r->worker.join();
     put_header();
-    const unsigned phase = pendsize ? (bp & 7u) : 0u;
+    const unsigned phase = staging->phase();
     std::vector<Engine::EmitPiece> ep;
     std::vector<uint64_t> ub;
     const uint64_t end = place_pieces(r->sr.pieces, r->base, phase, ep, &ub, opt.verbose != 0);
@@ -489,26 +550,23 @@ struct ZopfliB200Compressor {
       index.push_back({r->sr.pieces[m].instart - dict_len,
                        header_bytes + (deflate_bits - phase + stored_end(ep[m].bit_start, 0)) / 8});
     deflate_bits += end - phase;
-    splice_pieces(r->sr.recs, r->sr.stored.data(), &bp, &pend, &pendsize);
+    staging->splice(r->slot, r->base, r->sr);
+    staging->drop_records(r->sr);
     const uint64_t n = r->w.b - r->w.a;
     if (kind == kCkCrc32) sum = crc32_combine(sum, r->sum, n);
     else if (kind == kCkAdler32) sum = adler32_combine(sum, r->sum, n);
     free_slots.push_back(r->slot);
   }
 
-  // appends the complete bytes (all of them with `all`) to the caller's buffer
-  // appends the complete bytes (all of them with `all`) to the caller's buffer.  What stays behind is at most
-  // the partly filled last byte, in a fresh one-byte buffer: zopfli's capacity rule derives a buffer's
-  // capacity from its size, so a larger buffer must not be kept under a smaller size.
-  void hand_out(unsigned char** out, size_t* outsize, bool all) {
-    const size_t keep = (!all && bp != 0 && pendsize > 0) ? 1 : 0;
-    const unsigned char last = keep ? pend[pendsize - 1] : 0;
-    append_bytes(pend, pendsize - keep, out, outsize);
-    produced += pendsize - keep;
-    free(pend);
-    pend = nullptr;
-    pendsize = 0;
-    if (keep) append_bytes(&last, 1, &pend, &pendsize);
+  // the complete bytes (all of them with `all`) to the caller: appended to a host buffer, or with to_device a
+  // fresh device allocation
+  void hand_out(unsigned char** out, size_t* outsize, bool all, bool to_device) {
+    produced += staging->hand_out(all, to_device, out, outsize);
+  }
+
+  // what every output call refuses: no place for the output, a finished compressor, device output of a host one
+  bool refuses(unsigned char** out, size_t* outsize, bool to_device) const {
+    return !out || !outsize || finished || (to_device && staging->device() < 0);
   }
 
   int set_dictionary(const unsigned char* dict, size_t n) {
@@ -531,11 +589,10 @@ struct ZopfliB200Compressor {
   void put_marker(bool full) {
     while (!inflight.empty()) retire_oldest();
     put_header();
-    SpanPiece marker;
-    marker.stored = true;
-    marker.final = false;
-    marker.instart = marker.inend = 0;
-    splice_pieces({marker}, nullptr, &bp, &pend, &pendsize);
+    SpanRecords marker;
+    marker.recs.resize(1);
+    marker.recs[0].stored = true;
+    staging->splice(-1, 0, marker);
     deflate_bits = stored_end(deflate_bits, 0);
     if (!full) return;
     floor = received;
@@ -560,8 +617,8 @@ struct ZopfliB200Compressor {
     return k;
   }
 
-  int write(const unsigned char* chunk, size_t n, unsigned char** out, size_t* outsize) {
-    if (!out || !outsize || finished || !staging->accepts(chunk, n)) return 1;
+  int write(const unsigned char* chunk, size_t n, unsigned char** out, size_t* outsize, bool to_device) {
+    if (refuses(out, outsize, to_device) || !staging->accepts(chunk, n)) return 1;
     const double t0 = now_ms();
     started = true;
     if (n) {
@@ -579,15 +636,15 @@ struct ZopfliB200Compressor {
       fill_to(total, chunk, at);
     }
     while (!inflight.empty() && inflight.front()->done) retire_oldest();
-    hand_out(out, outsize, false);
+    hand_out(out, outsize, false, to_device);
     busy_ms += now_ms() - t0;
     return 0;
   }
 
   // mode 2 (sync) or 3 (full): what is left becomes one wave, then the marker, a stored block of BFINAL 0 and
   // LEN 0 (ZopfliDeflatePart with btype 0 over an empty range, deflate.c:625-663); the stream is byte-aligned
-  int flush(int mode, unsigned char** out, size_t* outsize) {
-    if (!out || !outsize || finished || (mode != 2 && mode != 3)) return 1;
+  int flush(int mode, unsigned char** out, size_t* outsize, bool to_device) {
+    if (refuses(out, outsize, to_device) || (mode != 2 && mode != 3)) return 1;
     const double t0 = now_ms();
     started = true;
     Wave w;
@@ -596,13 +653,13 @@ struct ZopfliB200Compressor {
       launch(w);
     }
     put_marker(mode == 3);
-    hand_out(out, outsize, true);
+    hand_out(out, outsize, true, to_device);
     busy_ms += now_ms() - t0;
     return 0;
   }
 
-  int finish(unsigned char** out, size_t* outsize) {
-    if (!out || !outsize || finished) return 1;
+  int finish(unsigned char** out, size_t* outsize, bool to_device) {
+    if (refuses(out, outsize, to_device)) return 1;
     const double t0 = now_ms();
     finished = true;
     Wave w;
@@ -611,8 +668,8 @@ struct ZopfliB200Compressor {
     while (!inflight.empty()) retire_oldest();
     const size_t insize = received - dict_len;
     unsigned char tr[8];
-    append_bytes(tr, container_trailer(kind, sum, insize, tr), &pend, &pendsize);
-    hand_out(out, outsize, true);
+    staging->put_bytes(tr, container_trailer(kind, sum, insize, tr));
+    hand_out(out, outsize, true, to_device);
     if (opt.verbose) report_sizes(fmt, insize, (size_t)((deflate_bits + 7) / 8), produced);
     layout.push_back(deflate_bits);
     busy_ms += now_ms() - t0;
@@ -698,8 +755,8 @@ int ZopfliB200DeflateSpan(const ZopfliOptions* options, const unsigned char* in,
     eng->set_input_host(in + base, end - base);
   }
   SpanRecords sr;
-  deflate_span_records(*eng, options, base, master_blocks(start, end), final != 0,
-                       [&](size_t pos, size_t n, unsigned char* dst) { memcpy(dst, in + pos, n); }, sr);
+  deflate_span_records(*eng, options, base, master_blocks(start, end), final != 0, sr);
+  span_records_to_host(*eng, sr, [&](size_t pos, size_t n, unsigned char* dst) { memcpy(dst, in + pos, n); });
   size_t total = 0;
   for (const SpanPiece& r : sr.recs) total += 10 + (r.stored ? r.inend - r.instart : r.bits.bytes.size());
   unsigned char* d = append_reserve(total, span, spansize);
@@ -727,37 +784,7 @@ int ZopfliB200AppendSpan(const unsigned char* span, size_t spansize, unsigned ch
                          size_t* outsize) {
   std::vector<SpanPiece> pieces;
   std::vector<unsigned char> rawbytes;  // stored payloads, addressed through instart/inend
-  size_t o = 0;
-  // validate the whole span before touching the output: spans arrive over a transport
-  while (o < spansize) {
-    if (spansize - o < 10 || span[o] > 1 || span[o + 1] > 1) return 1;
-    uint64_t v;
-    memcpy(&v, span + o + 2, 8);
-    const uint64_t nbytes = span[o] == 1 ? v : (v + 7) / 8;
-    if (nbytes > spansize - o - 10) return 1;
-    o += 10 + (size_t)nbytes;
-  }
-  o = 0;
-  // first pass: collect stored payloads contiguously so Piece offsets can index one buffer
-  while (o + 10 <= spansize) {
-    uint64_t v;
-    memcpy(&v, span + o + 2, 8);
-    bool stored = span[o] == 1;
-    size_t nbytes = stored ? (size_t)v : (size_t)((v + 7) / 8);
-    SpanPiece p;
-    p.stored = stored;
-    p.final = span[o + 1] != 0;
-    if (stored) {
-      p.instart = rawbytes.size();
-      rawbytes.insert(rawbytes.end(), span + o + 10, span + o + 10 + nbytes);
-      p.inend = rawbytes.size();
-    } else {
-      p.bits.bytes.assign(span + o + 10, span + o + 10 + nbytes);
-      p.bits.nbits = v;
-    }
-    pieces.push_back(std::move(p));
-    o += 10 + nbytes;
-  }
+  if (!parse_span(span, spansize, pieces, rawbytes)) return 1;
   splice_pieces(pieces, rawbytes.data(), bp, out, outsize);
   return 0;
 }
@@ -775,15 +802,28 @@ int ZopfliB200CompressorNew(const ZopfliOptions* options, ZopfliFormat output_ty
 
 int ZopfliB200CompressorWrite(ZopfliB200Compressor* c, const unsigned char* chunk, size_t n, unsigned char** out,
                               size_t* outsize) {
-  return c ? c->write(chunk, n, out, outsize) : 1;
+  return c ? c->write(chunk, n, out, outsize, false) : 1;
 }
 
 int ZopfliB200CompressorFinish(ZopfliB200Compressor* c, unsigned char** out, size_t* outsize) {
-  return c ? c->finish(out, outsize) : 1;
+  return c ? c->finish(out, outsize, false) : 1;
 }
 
 int ZopfliB200CompressorFlush(ZopfliB200Compressor* c, int mode, unsigned char** out, size_t* outsize) {
-  return c ? c->flush(mode, out, outsize) : 1;
+  return c ? c->flush(mode, out, outsize, false) : 1;
+}
+
+int ZopfliB200CompressorWriteToDevice(ZopfliB200Compressor* c, const unsigned char* chunk, size_t n,
+                                      unsigned char** dev_out, size_t* outsize) {
+  return c ? c->write(chunk, n, dev_out, outsize, true) : 1;
+}
+
+int ZopfliB200CompressorFlushToDevice(ZopfliB200Compressor* c, int mode, unsigned char** dev_out, size_t* outsize) {
+  return c ? c->flush(mode, dev_out, outsize, true) : 1;
+}
+
+int ZopfliB200CompressorFinishToDevice(ZopfliB200Compressor* c, unsigned char** dev_out, size_t* outsize) {
+  return c ? c->finish(dev_out, outsize, true) : 1;
 }
 
 int ZopfliB200CompressorSetDictionary(ZopfliB200Compressor* c, const unsigned char* dict, size_t n) {

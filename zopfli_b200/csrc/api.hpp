@@ -19,14 +19,22 @@ class Engine;
 
 // ZopfliB200DeflateSpan's body: the units of the input (master blocks, each with its floor), whose bytes from
 // position `base` on the engine already holds, as span records; after every unit marked `restart` comes a sync
-// marker (an empty stored block of BFINAL 0).  read(pos, n, dst) copies input bytes [pos, pos + n) to the host:
-// the payloads of stored blocks.
+// marker (an empty stored block of BFINAL 0).  The runs of compressed blocks are laid out, not yet emitted.
 void deflate_span_records(Engine& eng, const ZopfliOptions* opt, size_t base, const std::vector<Unit>& units,
-                          bool final, const std::function<void(size_t, size_t, unsigned char*)>& read,
-                          SpanRecords& out);
+                          bool final, SpanRecords& out);
+// The records' bytes on the host: the runs emitted and downloaded, and the payloads of stored blocks, which
+// read(pos, n, dst) copies from input bytes [pos, pos + n).
+void span_records_to_host(Engine& eng, SpanRecords& sr, const std::function<void(size_t, size_t, unsigned char*)>& read);
 
-// Where a compressor (ZopfliB200Compressor) keeps the bytes of its waves: host memory here, device memory in
-// device_api.cpp.  Slot s holds stream bytes from the slot's base on; it grows as bytes are put into it.
+// A span of ZopfliB200AppendSpan's format as records (stored payloads concatenated in rawbytes, addressed
+// through instart / inend); false, with nothing parsed, when it is malformed.
+struct SpanPiece;
+bool parse_span(const unsigned char* span, size_t spansize, std::vector<SpanPiece>& pieces,
+                std::vector<unsigned char>& rawbytes);
+
+// Where a compressor (ZopfliB200Compressor) keeps the bytes of its waves and of the stream it has not returned
+// yet: host memory here, device memory in device_api.cpp.  Slot s holds stream bytes from the slot's base on;
+// it grows as bytes are put into it.
 struct WaveStaging {
   static constexpr int kSlots = 3;  // two waves in flight and one filling
   size_t slot_bytes = 0;            // the most a slot holds: one wave and its dictionary (set by the compressor)
@@ -42,10 +50,25 @@ struct WaveStaging {
   virtual void stage(Engine& eng, int s, size_t len) = 0;
   // CRC-32 / Adler-32 (ChecksumKind) of slot s's bytes [off, off + n), with the engine set up by stage()
   virtual uint32_t checksum(Engine& eng, int s, size_t off, size_t n, int kind) = 0;
-  // slot s's bytes [off, off + n) to dst
-  virtual void read(Engine& eng, int s, size_t off, size_t n, unsigned char* dst) = 0;
+  // on a wave's worker, holding eng: the bytes of slot s's records (base: position of the slot's byte 0) where
+  // splice() reads them.  Host: downloaded runs and copied payloads; device: the runs in an allocation of
+  // sr.dev_runs, payloads left in the slot, which the wave holds until it is spliced.
+  virtual void take_records(Engine& eng, int s, size_t base, SpanRecords& sr) = 0;
+  // frees what take_records allocated
+  virtual void drop_records(SpanRecords& sr) = 0;
   // CRC-32 / Adler-32 of n bytes at p, memory of the kind this staging takes (a preset dictionary)
   virtual uint32_t checksum_of(const unsigned char* p, size_t n, int kind) = 0;
+
+  // ---- the stream not yet returned: at most the partly filled last byte between calls ----
+  // bits in use in the stream's last byte (0: none, or it is full)
+  virtual unsigned phase() const = 0;
+  // n whole bytes behind the stream's last byte (the container header and trailer)
+  virtual void put_bytes(const unsigned char* p, size_t n) = 0;
+  // records at the stream's bit phase; their bytes are where take_records left them (slot s from position base)
+  virtual void splice(int s, size_t base, const SpanRecords& sr) = 0;
+  // Returns the complete bytes (all of them with `all`) and their count: appended zopfli-style to *out, or with
+  // to_device (device staging only) as a fresh allocation *out of exactly *outsize bytes, NULL when there are none.
+  virtual size_t hand_out(bool all, bool to_device, unsigned char** out, size_t* outsize) = 0;
 };
 // The device side of ZopfliB200CompressorNew, registered by device_api.cpp (null in a host-only build): a
 // staging on device dev, ordered after cuda_stream, or null when dev is not a usable device.

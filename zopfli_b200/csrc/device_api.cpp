@@ -3,6 +3,8 @@
 // is emitted behind the container header in a device allocation, and the checksum is computed on the device.
 // Also the device half of the block-emission seam (ZopfliB200DeviceEmitBlocks) and the device staging of
 // ZopfliB200Compressor, which need engine calls the host-only test build of api.cpp does not have.
+#include <string.h>
+
 #include <algorithm>
 #include <vector>
 
@@ -55,18 +57,25 @@ int device_checksum(const unsigned char* dev_in, size_t size, void* stream, int 
 
 // A compressor's waves in device memory (chunks of one device): one stream-ordered allocation per slot, grown
 // as bytes arrive up to one wave and its dictionary.  Each chunk is copied device to device after the work
-// queued on the caller's stream; a wave's engine adopts its slot as input (no host copy), and only the bytes of
-// stored blocks come back to the host.
+// queued on the caller's stream; a wave's engine adopts its slot as input (no host copy).  The stream stays on
+// the device too: each wave's runs of compressed blocks are emitted into an allocation of their own, and k_splice
+// places them and the stored blocks (read from the slot) on the pending stream, so only the bytes a caller asks
+// for on the host are downloaded.
 struct DeviceWaveStaging : WaveStaging {
   DeviceStaging ds;
   void* user_stream;
   unsigned char* slot[kSlots] = {};
   size_t cap[kSlots] = {}, len[kSlots] = {};
   static constexpr size_t kPad = 64;  // the kernels read up to 16 bytes past the input; zeroed as set_input_host does
+  // the stream not yet returned: pend_bits bits from bit 0 of pend, which is zero past them
+  unsigned char* pend = nullptr;
+  size_t pend_cap = 0;
+  uint64_t pend_bits = 0;
 
   DeviceWaveStaging(int dev, void* stream) : ds(dev), user_stream(stream) {}
   ~DeviceWaveStaging() override {
     for (int s = 0; s < kSlots; s++) ds.release(slot[s]);
+    ds.release(pend);
   }
   int device() const override { return ds.device(); }
   bool accepts(const void* p, size_t n) const override { return n == 0 || Engine::pointer_device(p) == ds.device(); }
@@ -101,12 +110,149 @@ struct DeviceWaveStaging : WaveStaging {
   uint32_t checksum(Engine& eng, int s, size_t off, size_t n, int kind) override {
     return eng.checksum_device(slot[s] + off, n, ds.stream(), kind);
   }
-  void read(Engine& eng, int s, size_t off, size_t n, unsigned char* dst) override { eng.download(slot[s] + off, dst, n); }
+  void take_records(Engine& eng, int, size_t, SpanRecords& sr) override {
+    if (!sr.run_bits) return;
+    const void* bits = eng.emit_device(sr.ep, sr.run_bits, 0);  // done when it returns
+    const size_t n = (size_t)(sr.run_bits / 8);  // whole 8-byte words: every run starts on one
+    sr.dev_runs = (unsigned char*)ds.alloc(n);
+    ds.copy(sr.dev_runs, bits, n, ds.stream());
+  }
+  void drop_records(SpanRecords& sr) override {
+    ds.release(sr.dev_runs);
+    sr.dev_runs = nullptr;
+  }
   uint32_t checksum_of(const unsigned char* p, size_t n, int kind) override {  // k_crc32 / k_adler32: no PCIe copy
     Engine::Lease eng(ds.device());
     return eng->checksum_device(p, n, user_stream, kind);
   }
+
+  unsigned phase() const override { return (unsigned)(pend_bits & 7); }
+  // room for a stream of end_bits bits in whole 4-byte words (k_splice's unit), zero past the current stream
+  void pend_grow(uint64_t end_bits) {
+    const size_t need = (size_t)((end_bits + 31) / 32) * 4;
+    if (need <= pend_cap) return;
+    const size_t want = std::max(need, 2 * pend_cap);
+    unsigned char* p = (unsigned char*)ds.alloc(want);
+    ds.zero(p, want);
+    if (pend) {
+      ds.copy(p, pend, (size_t)((pend_bits + 7) / 8), ds.stream());
+      ds.release(pend);
+    }
+    pend = p;
+    pend_cap = want;
+  }
+  void put(const std::vector<Engine::SplicePiece>& recs, uint64_t end) {
+    pend_grow(end);
+    Engine::Lease eng(ds.device());  // for this splice only: the compressor holds no context between calls
+    eng->splice(recs, pend, ds.stream());
+    pend_bits = end;
+  }
+  void put_bytes(const unsigned char* p, size_t n) override {
+    if (n == 0) return;
+    Engine::SplicePiece r;
+    memset(&r, 0, sizeof(r));
+    r.bit_start = (pend_bits + 7) & ~(uint64_t)7;
+    r.nbits = (uint64_t)n * 8;
+    r.src = p;
+    r.literal = 1;
+    put({r}, r.bit_start + r.nbits);
+  }
+  void splice(int s, size_t base, const SpanRecords& sr) override {
+    std::vector<uint64_t> start;
+    const uint64_t end = span_positions(sr.recs, pend_bits, start);  // the placement splice_pieces uses
+    std::vector<Engine::SplicePiece> recs(sr.recs.size());
+    for (size_t i = 0; i < recs.size(); i++) {
+      const SpanPiece& p = sr.recs[i];
+      Engine::SplicePiece& r = recs[i];
+      memset(&r, 0, sizeof(r));
+      r.bit_start = start[i];
+      if (p.stored) {
+        r.stored = 1;
+        r.final = p.final ? 1 : 0;
+        r.len = p.inend - p.instart;
+        r.src = r.len ? slot[s] + (p.src - base) : nullptr;
+      } else {
+        r.nbits = p.bits.nbits;
+        r.src = sr.dev_runs + p.src / 8;
+      }
+    }
+    put(recs, end);
+  }
+  size_t hand_out(bool all, bool to_device, unsigned char** out, size_t* outsize) override {
+    const size_t used = (size_t)((pend_bits + 7) / 8), n = all ? used : (size_t)(pend_bits / 8);
+    if (to_device) {
+      *out = nullptr;
+      *outsize = 0;
+    }
+    if (n && to_device) {
+      *out = (unsigned char*)ds.alloc_on(n, user_stream);
+      ds.copy(*out, pend, n, user_stream);  // after the allocation; done when it returns
+      *outsize = n;
+    } else if (n) {
+      Engine::Lease eng(ds.device());
+      eng->download(pend, append_reserve(n, out, outsize), n);
+    }
+    // the partly filled last byte, if it stays, moves to byte 0; the rest is zero again
+    const size_t keep = used - n;
+    if (keep && n) ds.copy(pend, pend + n, 1, ds.stream());
+    if (used > keep) ds.zero(pend + keep, used - keep);
+    pend_bits -= (uint64_t)n * 8;
+    return n;
+  }
 };
+
+// ZopfliB200AppendSpan with the splice done by k_splice: the records' bytes (each from a 4-byte boundary) and the
+// caller's partly filled last byte are uploaded, spliced on the device, and the new bytes downloaded
+int device_append_span(const unsigned char* span, size_t spansize, unsigned char* bp, unsigned char** out,
+                       size_t* outsize) {
+  std::vector<SpanPiece> pieces;
+  std::vector<unsigned char> raw;
+  if (!bp || !out || !outsize || !parse_span(span, spansize, pieces, raw)) return 1;
+  const unsigned phase = (*outsize > 0) ? *bp : 0u;  // splice_pieces' bit0
+  if (phase > 7) return 1;
+  std::vector<uint64_t> start;
+  const uint64_t end = span_positions(pieces, phase, start);
+  const size_t nbytes = (size_t)((end + 7) / 8);
+  if (pieces.empty() || nbytes == 0) {
+    *bp = (unsigned char)(end & 7);
+    return 0;
+  }
+  std::vector<size_t> at(pieces.size());
+  std::vector<unsigned char> src;
+  for (size_t i = 0; i < pieces.size(); i++) {
+    const SpanPiece& p = pieces[i];
+    at[i] = src.size();
+    if (p.stored) src.insert(src.end(), raw.begin() + p.instart, raw.begin() + p.inend);
+    else src.insert(src.end(), p.bits.bytes.begin(), p.bits.bytes.end());
+    src.resize((src.size() + 3) & ~(size_t)3);
+  }
+  const int dev = Engine::current_device();
+  DeviceStaging ds(dev);
+  const size_t cap = (nbytes + 3) & ~(size_t)3;
+  unsigned char* d_src = (unsigned char*)ds.alloc(src.size() + 4);
+  unsigned char* d_out = (unsigned char*)ds.alloc(cap);
+  ds.zero(d_out, cap);
+  Engine::Lease eng(dev);
+  if (!src.empty()) eng->upload(d_src, src.data(), src.size());
+  if (phase) eng->upload(d_out, *out + *outsize - 1, 1);
+  std::vector<Engine::SplicePiece> recs(pieces.size());
+  for (size_t i = 0; i < pieces.size(); i++) {
+    Engine::SplicePiece& r = recs[i];
+    memset(&r, 0, sizeof(r));
+    r.bit_start = start[i];
+    r.src = d_src + at[i];
+    r.stored = pieces[i].stored ? 1 : 0;
+    r.final = pieces[i].final ? 1 : 0;
+    r.len = pieces[i].inend - pieces[i].instart;
+    r.nbits = pieces[i].bits.nbits;
+  }
+  eng->splice(recs, d_out, ds.stream());
+  append_stream(nbytes, phase, out, outsize, [&](unsigned char* dst) { eng->download(d_out, dst, nbytes); });
+  ds.release(d_src);
+  ds.release(d_out);
+  *bp = (unsigned char)(end & 7);
+  return 0;
+}
 
 WaveStaging* device_staging(int dev, void* stream) {
   if (dev < 0 || dev >= Engine::device_count()) return nullptr;
@@ -137,6 +283,11 @@ int ZopfliB200Crc32Device(const unsigned char* dev_in, size_t size, void* cuda_s
 
 int ZopfliB200Adler32Device(const unsigned char* dev_in, size_t size, void* cuda_stream, uint32_t* adler) {
   return device_checksum(dev_in, size, cuda_stream, kCkAdler32, adler);
+}
+
+int ZopfliB200DeviceAppendSpan(const unsigned char* span, size_t spansize, unsigned char* bp, unsigned char** out,
+                               size_t* outsize) {
+  return device_append_span(span, spansize, bp, out, outsize);
 }
 
 int ZopfliB200DeviceProbeParts(const uint32_t* hists, size_t nhist, uint32_t* smoothed, unsigned char* lengths,

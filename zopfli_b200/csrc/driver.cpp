@@ -662,12 +662,9 @@ void append_bytes(const unsigned char* src, size_t n, unsigned char** out, size_
 // Every piece's bit offset follows from a prefix sum over the piece sizes, so the pieces are copied
 // (shifted by their bit phase) in parallel straight into the output buffer; only the bytes shared
 // between neighbouring pieces are merged serially.
-void splice_pieces(const std::vector<SpanPiece>& pieces, const unsigned char* in, unsigned char* bp,
-                   unsigned char** out, size_t* outsize) {
+uint64_t span_positions(const std::vector<SpanPiece>& pieces, uint64_t bit0, std::vector<uint64_t>& start) {
   const size_t np = pieces.size();
-  uint64_t bit0 = (uint64_t)*outsize * 8;
-  if (*bp != 0 && *outsize > 0) bit0 = (uint64_t)(*outsize - 1) * 8 + *bp;
-  std::vector<uint64_t> start(np + 1);
+  start.resize(np + 1);
   uint64_t pos = bit0;
   for (size_t i = 0; i < np; i++) {
     const SpanPiece& p = pieces[i];
@@ -675,6 +672,16 @@ void splice_pieces(const std::vector<SpanPiece>& pieces, const unsigned char* in
     pos = p.stored ? stored_end(pos, p.inend - p.instart) : pos + p.bits.nbits;
   }
   start[np] = pos;
+  return pos;
+}
+
+void splice_pieces(const std::vector<SpanPiece>& pieces, const unsigned char* in, unsigned char* bp,
+                   unsigned char** out, size_t* outsize) {
+  const size_t np = pieces.size();
+  uint64_t bit0 = (uint64_t)*outsize * 8;
+  if (*bp != 0 && *outsize > 0) bit0 = (uint64_t)(*outsize - 1) * 8 + *bp;
+  std::vector<uint64_t> start;
+  const uint64_t pos = span_positions(pieces, bit0, start);
   const size_t oldsize = *outsize, newsize = (size_t)((pos + 7) / 8);
   append_reserve(newsize - oldsize, out, outsize);  // one append of everything
   unsigned char* o = *out;

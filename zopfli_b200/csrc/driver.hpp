@@ -42,16 +42,24 @@ struct SpanPiece {
   BitString bits;
   size_t instart = 0, inend = 0;
   bool final = false;
+  // where the record's bytes come from (deflate_span_records): for bits, the first bit in the emission of the
+  // runs (SpanRecords::ep); stored, the input position of the payload
+  uint64_t src = 0;
 };
 
 // ZopfliB200DeflateSpan's records of a range of units: the driver's pieces, and the records made of them
 // (maximal runs of compressed pieces as bits, stored pieces as ranges of `stored`, their bytes).  `markers`
-// indexes the pieces that are full-flush markers after units that end at a restart point.
+// indexes the pieces that are full-flush markers after units that end at a restart point.  The runs are
+// emitted together (ep, run_bits bits): to the host by span_records_to_host, which fills bits.bytes and
+// `stored`, or by a device compressor into dev_runs, which it owns.
 struct SpanRecords {
   std::vector<Piece> pieces;
   std::vector<SpanPiece> recs;
   std::vector<unsigned char> stored;
   std::vector<size_t> markers;
+  std::vector<Engine::EmitPiece> ep;
+  uint64_t run_bits = 0;
+  unsigned char* dev_runs = nullptr;
 };
 
 struct HostTimes { double split = 0, emit = 0, other = 0; };
@@ -111,6 +119,10 @@ uint64_t place_pieces(const std::vector<Piece>& pieces, size_t in_base, unsigned
 // bit position of every piece when the first one starts at bit0; returns the end position
 uint64_t layout_pieces(const std::vector<Piece>& pieces, size_t in_base, uint64_t bit0, std::vector<Engine::EmitPiece>& ep,
                        std::vector<uint64_t>* unit_bits);
+
+// Where span records go when the first starts at bit0: start[i] for record i, start[n] = the end (returned).
+// The one placement of records, for the host splice below and the device splice (k_splice).
+uint64_t span_positions(const std::vector<SpanPiece>& pieces, uint64_t bit0, std::vector<uint64_t>& start);
 
 void splice_pieces(const std::vector<SpanPiece>& pieces, const unsigned char* in, unsigned char* bp,
                    unsigned char** out, size_t* outsize);

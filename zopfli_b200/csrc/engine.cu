@@ -1427,6 +1427,55 @@ uint8_t* Engine::emit_to_device(const std::vector<EmitPiece>& pieces, uint64_t t
   return out;
 }
 
+void Engine::splice(const std::vector<SplicePiece>& recs, uint8_t* dst, void* after_stream) {
+  Impl& m = *p_;
+  Lane& l = m.lane[0];
+  std::lock_guard<std::mutex> g(l.mu);
+  CK(cudaSetDevice(m.dev));
+  // descriptors, then one 16-byte slot per literal, in one upload
+  std::vector<SpliceDesc> d;
+  std::vector<std::pair<size_t, const SplicePiece*>> lits;  // (first descriptor, record)
+  for (const SplicePiece& r : recs) {
+    if (r.stored) {
+      uint64_t q = r.bit_start, left = r.len, off = 0;
+      do {  // the sub-blocks of write_stored, one CTA each
+        const uint64_t bs = left > 65535 ? 65535 : left;
+        left -= bs;
+        d.push_back(SpliceDesc{q, 0, r.src + off, bs, 1u | ((r.final && left == 0) ? 1u << 8 : 0u), 0});
+        q = stored_end(q, bs);
+        off += bs;
+      } while (left);
+      continue;
+    }
+    if (r.literal) {
+      if (r.nbits > 128) { fprintf(stderr, "zopfli-b200: literal splice record of %llu bits\n", (unsigned long long)r.nbits); abort(); }
+      lits.push_back({d.size(), &r});
+    }
+    for (uint64_t t = 0; t < r.nbits; t += kSpliceTileBits)
+      d.push_back(SpliceDesc{r.bit_start + t, std::min(kSpliceTileBits, r.nbits - t), r.src + t / 8, 0, 0, 0});
+  }
+  if (d.empty()) return;
+  const size_t desc_b = d.size() * sizeof(SpliceDesc), blob_b = desc_b + lits.size() * 16;
+  m.emit_desc.ensure(blob_b + 64);
+  std::vector<uint8_t> blob(blob_b, 0);
+  for (size_t i = 0; i < lits.size(); i++) {
+    const SplicePiece& r = *lits[i].second;
+    memcpy(blob.data() + desc_b + 16 * i, r.src, (size_t)((r.nbits + 7) / 8));
+    d[lits[i].first].src = (const uint8_t*)m.emit_desc.p + desc_b + 16 * i;
+  }
+  memcpy(blob.data(), d.data(), desc_b);
+  CK(cudaEventRecord(m.ev_user, (cudaStream_t)after_stream));
+  CK(cudaStreamWaitEvent(l.stream, m.ev_user, 0));
+  l.tic();
+  CK(cudaMemcpyAsync(m.emit_desc.p, blob.data(), blob_b, cudaMemcpyHostToDevice, l.stream));
+  k_splice<<<(unsigned)d.size(), kSpliceThreads, 0, l.stream>>>(m.emit_desc.as<SpliceDesc>(), (uint32_t*)dst);
+  CK(cudaGetLastError());
+  l.toc(l.acc.ms_pack);
+  l.sync();
+  l.acc.launches++;
+  l.acc.h2d_bytes += blob_b;
+}
+
 uint64_t Engine::device_block_bits(const uint32_t* hist320) {
   Impl& m = *p_;
   Lane& l = m.lane[0];
@@ -1499,6 +1548,13 @@ void* DeviceStaging::alloc(size_t bytes) {
   OnDevice on(dev_);
   void* p = nullptr;
   CK(cudaMallocAsync(&p, bytes, (cudaStream_t)stream_));
+  return p;
+}
+
+void* DeviceStaging::alloc_on(size_t bytes, void* user_stream) {
+  OnDevice on(dev_);
+  void* p = nullptr;
+  CK(cudaMallocAsync(&p, bytes, (cudaStream_t)user_stream));
   return p;
 }
 

@@ -137,6 +137,34 @@ struct WordSink {  // LSB-first bit writer for one thread: every word it touches
 constexpr int kEmitThreads = 256;
 constexpr int kEmitItems = 4;   // symbols per thread per round
 
+// AddNonCompressedBlock deflate.c:625-663, the one writer of stored blocks on the device: bytes [ip, ip + len) of
+// `in` as sub-blocks of at most 65,535 bytes from bit q of a zeroed stream, BFINAL on the last one when `final`.
+// The header's byte may be shared with the block before (its bit is ORed in); every later byte belongs to this
+// block alone and gets a plain store.  Called by all kThreads threads of the CTA.
+template <int kThreads>
+__device__ __forceinline__ void write_stored(uint32_t* __restrict__ out, uint64_t q, const uint8_t* __restrict__ in,
+                                             uint64_t ip, uint64_t len, uint32_t final, uint32_t tid) {
+  uint8_t* out8 = (uint8_t*)out;
+  uint64_t left = len;
+  do {
+    const uint64_t bs = left > 65535 ? 65535 : left;
+    const bool last = left == bs;
+    const uint64_t lenpos = (q + 3 + 7) >> 3;  // LEN starts at the next byte boundary after the 3 header bits
+    if (tid == 0) {
+      if (final && last) atomicOr(&out[q >> 5], 1u << (q & 31));  // BFINAL; BTYPE 00 and the padding are zero bits
+      const uint32_t nlen = (~(uint32_t)bs) & 0xffffu;
+      out8[lenpos] = (uint8_t)(bs & 255);
+      out8[lenpos + 1] = (uint8_t)(bs >> 8);
+      out8[lenpos + 2] = (uint8_t)(nlen & 255);
+      out8[lenpos + 3] = (uint8_t)(nlen >> 8);
+    }
+    for (uint64_t i = tid; i < bs; i += kThreads) out8[lenpos + 4 + i] = in[ip + i];
+    q = (lenpos + 4 + bs) * 8;
+    ip += bs;
+    left -= bs;
+  } while (left);
+}
+
 __global__ void __launch_bounds__(kEmitThreads) k_emit(const EmitDesc* __restrict__ pieces, const uint8_t* __restrict__ in,
                                                        uint32_t* __restrict__ out, uint32_t* __restrict__ err) {
   __shared__ uint8_t ll_len[kNumLL], d_len[kNumD];
@@ -147,26 +175,8 @@ __global__ void __launch_bounds__(kEmitThreads) k_emit(const EmitDesc* __restric
   const uint32_t tid = threadIdx.x, lane = tid & 31u, wid = tid >> 5;
   const uint32_t type = p.type_final & 255u, final = p.type_final >> 8;
 
-  if (type == 0) {  // AddNonCompressedBlock deflate.c:625-663
-    uint8_t* out8 = (uint8_t*)out;
-    uint64_t q = p.bit_start, left = p.in_len, ip = p.in_start;
-    do {
-      const uint64_t bs = left > 65535 ? 65535 : left;
-      const bool last = left == bs;
-      const uint64_t lenpos = (q + 3 + 7) >> 3;  // LEN starts at the next byte boundary after the 3 header bits
-      if (tid == 0) {
-        if (final && last) atomicOr(&out[q >> 5], 1u << (q & 31));  // BFINAL; BTYPE 00 and the padding are zero bits
-        const uint32_t nlen = (~(uint32_t)bs) & 0xffffu;
-        out8[lenpos] = (uint8_t)(bs & 255);
-        out8[lenpos + 1] = (uint8_t)(bs >> 8);
-        out8[lenpos + 2] = (uint8_t)(nlen & 255);
-        out8[lenpos + 3] = (uint8_t)(nlen >> 8);
-      }
-      for (uint64_t i = tid; i < bs; i += kEmitThreads) out8[lenpos + 4 + i] = in[ip + i];
-      q = (lenpos + 4 + bs) * 8;
-      ip += bs;
-      left -= bs;
-    } while (left);
+  if (type == 0) {
+    write_stored<kEmitThreads>(out, p.bit_start, in, p.in_start, p.in_len, final, tid);
     return;
   }
 
@@ -249,6 +259,53 @@ __global__ void __launch_bounds__(kEmitThreads) k_emit(const EmitDesc* __restric
     WordSink sink{out, run};
     sink.put(ll_code[256], ll_len[256]);  // end code (deflate.c:718-719)
     if (sink.pos - p.bit_start != p.nbits) atomicExch(err, 0x80000000u | blockIdx.x);
+  }
+}
+
+// ---- k_splice: span records at absolute bit positions of a stream (a device compressor's pending bytes) ----
+// The destination is zero from its first bit on, as k_emit's is.  A bit record is a tile of at most
+// kSpliceTileBits bits that start at bit 0 of src (4-byte aligned, readable to the end of the tile's last word);
+// the host cuts longer records into tiles.  A stored record is one sub-block of at most 65,535 bytes (the host
+// cuts longer ones at the same boundaries write_stored does), written by write_stored.
+struct SpliceDesc {
+  uint64_t bit_start;       // absolute bit position in the destination
+  uint64_t nbits;           // bit records: bits of the tile
+  const uint8_t* src;       // bit records: the tile's bits; stored records: the payload
+  uint64_t len;             // stored records: payload bytes
+  uint32_t stored_final;    // 1 for a stored record | BFINAL << 8
+  uint32_t pad;
+};
+
+constexpr int kSpliceThreads = 256;
+constexpr uint64_t kSpliceTileBits = 32ull * kSpliceThreads * 8;  // 8 words per thread
+
+__global__ void __launch_bounds__(kSpliceThreads) k_splice(const SpliceDesc* __restrict__ recs, uint32_t* __restrict__ out) {
+  const SpliceDesc r = recs[blockIdx.x];
+  const uint32_t tid = threadIdx.x;
+  if (r.stored_final & 1u) {
+    write_stored<kSpliceThreads>(out, r.bit_start, r.src, 0, r.len, r.stored_final >> 8, tid);
+    return;
+  }
+  if (r.nbits == 0) return;
+  const uint32_t* s = (const uint32_t*)r.src;
+  const uint64_t nw = (r.nbits + 31) >> 5;  // source words
+  const uint32_t tail = (uint32_t)(r.nbits & 31);
+  const uint32_t sh = (uint32_t)(r.bit_start & 31);
+  const uint64_t w0 = r.bit_start >> 5, w1 = (r.bit_start + r.nbits - 1) >> 5;
+  auto word = [&](uint64_t k) -> uint32_t {  // source word k, zero past the record's last bit
+    if (k >= nw) return 0u;
+    const uint32_t v = s[k];
+    return (k + 1 == nw && tail) ? (v & ((1u << tail) - 1u)) : v;
+  };
+  // destination word w0 + k holds source bits [32k - sh, 32k - sh + 32)
+  for (uint64_t k = tid; w0 + k <= w1; k += kSpliceThreads) {
+    uint32_t v = word(k) << sh;
+    if (sh && k) v |= word(k - 1) >> (32 - sh);
+    if (k == 0 || w0 + k == w1) {  // the first and the last word may be shared with neighbours
+      if (v) atomicOr(out + w0 + k, v);
+    } else {
+      out[w0 + k] = v;  // a word strictly inside the record belongs to it alone
+    }
   }
 }
 
