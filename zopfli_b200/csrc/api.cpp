@@ -142,20 +142,18 @@ void deflate_span_records(Engine& eng, const ZopfliOptions* opt, size_t base, co
     }
   }
   // Records: maximal runs of compressed pieces, each emitted on the device from bit offset 0 of a
-  // byte-aligned slot of one buffer, and stored pieces as raw bytes.
+  // byte-aligned slot of one buffer, and stored pieces as their payload in the input.
   out.ep.clear();
+  out.at.clear();
   uint64_t pos = 0;
-  size_t nstored = 0;
   for (size_t i = 0; i < pieces.size();) {
-    SpanPiece r;
+    Engine::SpanRecord r;
     if (pieces[i].type == 0) {
       r.stored = true;
       r.final = pieces[i].final;
-      r.instart = nstored;
-      nstored += pieces[i].inend - pieces[i].instart;
-      r.inend = nstored;
-      r.src = pieces[i].instart;
-      out.recs.push_back(std::move(r));
+      r.n = pieces[i].inend - pieces[i].instart;
+      out.recs.push_back(r);
+      out.at.push_back(pieces[i].instart);
       i++;
       continue;
     }
@@ -165,35 +163,25 @@ void deflate_span_records(Engine& eng, const ZopfliOptions* opt, size_t base, co
     std::vector<Engine::EmitPiece> ep;
     const uint64_t e = layout_pieces(run, base, pos, ep, nullptr);
     r.final = pieces[j - 1].final;
-    r.bits.nbits = e - pos;
-    r.src = pos;
-    out.recs.push_back(std::move(r));
+    r.n = e - pos;
+    out.recs.push_back(r);
+    out.at.push_back(pos);
     out.ep.insert(out.ep.end(), ep.begin(), ep.end());
     pos = (e + 63) & ~(uint64_t)63;  // the next run starts on a fresh word: no shared bytes between records
     i = j;
   }
   out.run_bits = pos;
-  out.stored.clear();
 }
 
-void span_records_to_host(Engine& eng, SpanRecords& sr, const std::function<void(size_t, size_t, unsigned char*)>& read) {
-  std::vector<unsigned char> bits((size_t)(sr.run_bits / 8) + 8, 0);
-  if (sr.run_bits) eng.emit(sr.ep, sr.run_bits, bits.data());
-  size_t nstored = 0;
-  for (const SpanPiece& r : sr.recs) nstored = r.stored ? r.inend : nstored;
-  sr.stored.resize(nstored);
-  for (SpanPiece& r : sr.recs) {
-    if (!r.stored) {
-      const unsigned char* s = bits.data() + r.src / 8;
-      r.bits.bytes.assign(s, s + (size_t)((r.bits.nbits + 7) / 8));
-    } else if (r.inend > r.instart) {
-      read((size_t)r.src, r.inend - r.instart, sr.stored.data() + r.instart);
-    }
+void point_records(SpanRecords& sr, const unsigned char* runs, const unsigned char* in, size_t base) {
+  for (size_t i = 0; i < sr.recs.size(); i++) {
+    Engine::SpanRecord& r = sr.recs[i];
+    if (!r.stored) r.src = runs + sr.at[i] / 8;
+    else r.src = r.n ? in + (sr.at[i] - base) : nullptr;  // an empty one (a marker) reads nothing
   }
 }
 
-bool parse_span(const unsigned char* span, size_t spansize, std::vector<SpanPiece>& pieces,
-                std::vector<unsigned char>& rawbytes) {
+bool parse_span(const unsigned char* span, size_t spansize, std::vector<Engine::SpanRecord>& recs) {
   size_t o = 0;
   // validate the whole span before touching the output: spans arrive over a transport
   while (o < spansize) {
@@ -204,26 +192,14 @@ bool parse_span(const unsigned char* span, size_t spansize, std::vector<SpanPiec
     if (nbytes > spansize - o - 10) return false;
     o += 10 + (size_t)nbytes;
   }
-  o = 0;
-  // first pass: collect stored payloads contiguously so Piece offsets can index one buffer
-  while (o + 10 <= spansize) {
-    uint64_t v;
-    memcpy(&v, span + o + 2, 8);
-    bool stored = span[o] == 1;
-    size_t nbytes = stored ? (size_t)v : (size_t)((v + 7) / 8);
-    SpanPiece p;
-    p.stored = stored;
-    p.final = span[o + 1] != 0;
-    if (stored) {
-      p.instart = rawbytes.size();
-      rawbytes.insert(rawbytes.end(), span + o + 10, span + o + 10 + nbytes);
-      p.inend = rawbytes.size();
-    } else {
-      p.bits.bytes.assign(span + o + 10, span + o + 10 + nbytes);
-      p.bits.nbits = v;
-    }
-    pieces.push_back(std::move(p));
-    o += 10 + nbytes;
+  for (o = 0; o < spansize;) {
+    Engine::SpanRecord r;
+    r.stored = span[o] == 1;
+    r.final = span[o + 1] != 0;
+    r.src = span + o + 10;
+    memcpy(&r.n, span + o + 2, 8);
+    recs.push_back(r);
+    o += 10 + (size_t)(r.stored ? r.n : (r.n + 7) / 8);
   }
   return true;
 }
@@ -372,15 +348,23 @@ struct HostStaging : WaveStaging {
   uint32_t checksum(Engine&, int s, size_t off, size_t n, int kind) override {
     return host_checksum(at(s, off), n, kind, 0);
   }
+  // The records point into sr.runs and slot s until the wave is spliced: only the filling slot is written or
+  // regrown (put, carry), and slot s is not filling again before its wave is retired.
   void take_records(Engine& eng, int s, size_t base, SpanRecords& sr) override {
-    span_records_to_host(eng, sr, [&](size_t pos, size_t n, unsigned char* dst) { memcpy(dst, at(s, pos - base), n); });
+    sr.runs = (unsigned char*)calloc((size_t)(sr.run_bits / 8) + 8, 1);
+    if (!sr.runs) { fprintf(stderr, "zopfli-b200: out of memory\n"); exit(EXIT_FAILURE); }
+    if (sr.run_bits) eng.emit(sr.ep, sr.run_bits, sr.runs);
+    point_records(sr, sr.runs, slot[s].data(), base);
   }
-  void drop_records(SpanRecords&) override {}
+  void drop_records(SpanRecords& sr) override {
+    free(sr.runs);
+    sr.runs = nullptr;
+  }
   uint32_t checksum_of(const unsigned char* p, size_t n, int kind) override { return host_checksum(p, n, kind, 0); }
 
   unsigned phase() const override { return pendsize ? (bp & 7u) : 0u; }
   void put_bytes(const unsigned char* p, size_t n) override { append_bytes(p, n, &pend, &pendsize); }
-  void splice(int, size_t, const SpanRecords& sr) override { splice_pieces(sr.recs, sr.stored.data(), &bp, &pend, &pendsize); }
+  void splice(SpanRecords& sr) override { splice_pieces(sr.recs, &bp, &pend, &pendsize); }
   // What stays behind is at most the partly filled last byte, in a fresh one-byte buffer: zopfli's capacity rule
   // derives a buffer's capacity from its size, so a larger buffer must not be kept under a smaller size.
   size_t hand_out(bool all, bool, unsigned char** out, size_t* outsize) override {
@@ -550,7 +534,7 @@ struct ZopfliB200Compressor {
       index.push_back({r->sr.pieces[m].instart - dict_len,
                        header_bytes + (deflate_bits - phase + stored_end(ep[m].bit_start, 0)) / 8});
     deflate_bits += end - phase;
-    staging->splice(r->slot, r->base, r->sr);
+    staging->splice(r->sr);
     staging->drop_records(r->sr);
     const uint64_t n = r->w.b - r->w.a;
     if (kind == kCkCrc32) sum = crc32_combine(sum, r->sum, n);
@@ -592,7 +576,7 @@ struct ZopfliB200Compressor {
     SpanRecords marker;
     marker.recs.resize(1);
     marker.recs[0].stored = true;
-    staging->splice(-1, 0, marker);
+    staging->splice(marker);
     deflate_bits = stored_end(deflate_bits, 0);
     if (!full) return;
     floor = received;
@@ -756,17 +740,18 @@ int ZopfliB200DeflateSpan(const ZopfliOptions* options, const unsigned char* in,
   }
   SpanRecords sr;
   deflate_span_records(*eng, options, base, master_blocks(start, end), final != 0, sr);
-  span_records_to_host(*eng, sr, [&](size_t pos, size_t n, unsigned char* dst) { memcpy(dst, in + pos, n); });
+  std::vector<unsigned char> runs((size_t)(sr.run_bits / 8) + 8, 0);
+  if (sr.run_bits) eng->emit(sr.ep, sr.run_bits, runs.data());
+  point_records(sr, runs.data(), in, 0);
   size_t total = 0;
-  for (const SpanPiece& r : sr.recs) total += 10 + (r.stored ? r.inend - r.instart : r.bits.bytes.size());
+  for (const Engine::SpanRecord& r : sr.recs) total += 10 + (size_t)(r.stored ? r.n : (r.n + 7) / 8);
   unsigned char* d = append_reserve(total, span, spansize);
-  for (const SpanPiece& r : sr.recs) {
+  for (const Engine::SpanRecord& r : sr.recs) {
     d[0] = r.stored ? 1 : 0;
     d[1] = r.final ? 1 : 0;
-    const uint64_t v = r.stored ? (uint64_t)(r.inend - r.instart) : r.bits.nbits;
-    memcpy(d + 2, &v, 8);
-    const size_t nb = r.stored ? (size_t)v : r.bits.bytes.size();
-    if (nb) memcpy(d + 10, r.stored ? sr.stored.data() + r.instart : r.bits.bytes.data(), nb);
+    memcpy(d + 2, &r.n, 8);
+    const size_t nb = (size_t)(r.stored ? r.n : (r.n + 7) / 8);
+    if (nb) memcpy(d + 10, r.src, nb);
     d += 10 + nb;
   }
   return 0;
@@ -782,10 +767,9 @@ uint32_t ZopfliB200HostChecksumSliced(const unsigned char* data, size_t size, si
 
 int ZopfliB200AppendSpan(const unsigned char* span, size_t spansize, unsigned char* bp, unsigned char** out,
                          size_t* outsize) {
-  std::vector<SpanPiece> pieces;
-  std::vector<unsigned char> rawbytes;  // stored payloads, addressed through instart/inend
-  if (!parse_span(span, spansize, pieces, rawbytes)) return 1;
-  splice_pieces(pieces, rawbytes.data(), bp, out, outsize);
+  std::vector<Engine::SpanRecord> recs;
+  if (!parse_span(span, spansize, recs)) return 1;
+  splice_pieces(recs, bp, out, outsize);
   return 0;
 }
 

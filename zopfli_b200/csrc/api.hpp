@@ -4,10 +4,10 @@
 #include <stddef.h>
 #include <stdint.h>
 
-#include <functional>
 #include <vector>
 
 #include "../../include/zopfli.h"
+#include "engine.hpp"
 
 namespace zb {
 
@@ -15,22 +15,19 @@ struct BlockPlan;
 struct Piece;
 struct SpanRecords;
 struct Unit;
-class Engine;
 
 // ZopfliB200DeflateSpan's body: the units of the input (master blocks, each with its floor), whose bytes from
 // position `base` on the engine already holds, as span records; after every unit marked `restart` comes a sync
 // marker (an empty stored block of BFINAL 0).  The runs of compressed blocks are laid out, not yet emitted.
 void deflate_span_records(Engine& eng, const ZopfliOptions* opt, size_t base, const std::vector<Unit>& units,
                           bool final, SpanRecords& out);
-// The records' bytes on the host: the runs emitted and downloaded, and the payloads of stored blocks, which
-// read(pos, n, dst) copies from input bytes [pos, pos + n).
-void span_records_to_host(Engine& eng, SpanRecords& sr, const std::function<void(size_t, size_t, unsigned char*)>& read);
+// Points the records at their bytes once the runs are emitted: bit records into `runs`, the emission of sr.ep,
+// stored records at their payload in `in`, the input bytes from position `base` on.
+void point_records(SpanRecords& sr, const unsigned char* runs, const unsigned char* in, size_t base);
 
-// A span of ZopfliB200AppendSpan's format as records (stored payloads concatenated in rawbytes, addressed
-// through instart / inend); false, with nothing parsed, when it is malformed.
-struct SpanPiece;
-bool parse_span(const unsigned char* span, size_t spansize, std::vector<SpanPiece>& pieces,
-                std::vector<unsigned char>& rawbytes);
+// A span of ZopfliB200AppendSpan's format as records that point into it; false, with nothing parsed, when it
+// is malformed.
+bool parse_span(const unsigned char* span, size_t spansize, std::vector<Engine::SpanRecord>& recs);
 
 // Where a compressor (ZopfliB200Compressor) keeps the bytes of its waves and of the stream it has not returned
 // yet: host memory here, device memory in device_api.cpp.  Slot s holds stream bytes from the slot's base on;
@@ -50,9 +47,9 @@ struct WaveStaging {
   virtual void stage(Engine& eng, int s, size_t len) = 0;
   // CRC-32 / Adler-32 (ChecksumKind) of slot s's bytes [off, off + n), with the engine set up by stage()
   virtual uint32_t checksum(Engine& eng, int s, size_t off, size_t n, int kind) = 0;
-  // on a wave's worker, holding eng: the bytes of slot s's records (base: position of the slot's byte 0) where
-  // splice() reads them.  Host: downloaded runs and copied payloads; device: the runs in an allocation of
-  // sr.dev_runs, payloads left in the slot, which the wave holds until it is spliced.
+  // on a wave's worker, holding eng: emits the runs of slot s's records (base: position of the slot's byte 0)
+  // into a buffer of sr.runs, in memory of the staging's kind, and points the records there, stored ones at
+  // their payload in the slot.
   virtual void take_records(Engine& eng, int s, size_t base, SpanRecords& sr) = 0;
   // frees what take_records allocated
   virtual void drop_records(SpanRecords& sr) = 0;
@@ -64,8 +61,8 @@ struct WaveStaging {
   virtual unsigned phase() const = 0;
   // n whole bytes behind the stream's last byte (the container header and trailer)
   virtual void put_bytes(const unsigned char* p, size_t n) = 0;
-  // records at the stream's bit phase; their bytes are where take_records left them (slot s from position base)
-  virtual void splice(int s, size_t base, const SpanRecords& sr) = 0;
+  // records at the stream's bit phase, from the bytes take_records pointed them at
+  virtual void splice(SpanRecords& sr) = 0;
   // Returns the complete bytes (all of them with `all`) and their count: appended zopfli-style to *out, or with
   // to_device (device staging only) as a fresh allocation *out of exactly *outsize bytes, NULL when there are none.
   virtual size_t hand_out(bool all, bool to_device, unsigned char** out, size_t* outsize) = 0;

@@ -110,16 +110,20 @@ struct DeviceWaveStaging : WaveStaging {
   uint32_t checksum(Engine& eng, int s, size_t off, size_t n, int kind) override {
     return eng.checksum_device(slot[s] + off, n, ds.stream(), kind);
   }
-  void take_records(Engine& eng, int, size_t, SpanRecords& sr) override {
-    if (!sr.run_bits) return;
-    const void* bits = eng.emit_device(sr.ep, sr.run_bits, 0);  // done when it returns
-    const size_t n = (size_t)(sr.run_bits / 8);  // whole 8-byte words: every run starts on one
-    sr.dev_runs = (unsigned char*)ds.alloc(n);
-    ds.copy(sr.dev_runs, bits, n, ds.stream());
+  // The records point into sr.runs and slot s until the wave is spliced: only the filling slot is written or
+  // regrown (put, carry; stage grew slot s before this), and slot s is not filling again before its wave is retired.
+  void take_records(Engine& eng, int s, size_t base, SpanRecords& sr) override {
+    if (sr.run_bits) {
+      const void* bits = eng.emit_device(sr.ep, sr.run_bits, 0);  // done when it returns
+      const size_t n = (size_t)(sr.run_bits / 8);  // whole 8-byte words: every run starts on one
+      sr.runs = (unsigned char*)ds.alloc(n);
+      ds.copy(sr.runs, bits, n, ds.stream());
+    }
+    point_records(sr, sr.runs, slot[s], base);
   }
   void drop_records(SpanRecords& sr) override {
-    ds.release(sr.dev_runs);
-    sr.dev_runs = nullptr;
+    ds.release(sr.runs);
+    sr.runs = nullptr;
   }
   uint32_t checksum_of(const unsigned char* p, size_t n, int kind) override {  // k_crc32 / k_adler32: no PCIe copy
     Engine::Lease eng(ds.device());
@@ -141,7 +145,7 @@ struct DeviceWaveStaging : WaveStaging {
     pend = p;
     pend_cap = want;
   }
-  void put(const std::vector<Engine::SplicePiece>& recs, uint64_t end) {
+  void put(const std::vector<Engine::SpanRecord>& recs, uint64_t end) {
     pend_grow(end);
     Engine::Lease eng(ds.device());  // for this splice only: the compressor holds no context between calls
     eng->splice(recs, pend, ds.stream());
@@ -149,35 +153,14 @@ struct DeviceWaveStaging : WaveStaging {
   }
   void put_bytes(const unsigned char* p, size_t n) override {
     if (n == 0) return;
-    Engine::SplicePiece r;
-    memset(&r, 0, sizeof(r));
+    Engine::SpanRecord r;
     r.bit_start = (pend_bits + 7) & ~(uint64_t)7;
-    r.nbits = (uint64_t)n * 8;
+    r.n = (uint64_t)n * 8;
     r.src = p;
-    r.literal = 1;
-    put({r}, r.bit_start + r.nbits);
+    r.literal = true;
+    put({r}, r.bit_start + r.n);
   }
-  void splice(int s, size_t base, const SpanRecords& sr) override {
-    std::vector<uint64_t> start;
-    const uint64_t end = span_positions(sr.recs, pend_bits, start);  // the placement splice_pieces uses
-    std::vector<Engine::SplicePiece> recs(sr.recs.size());
-    for (size_t i = 0; i < recs.size(); i++) {
-      const SpanPiece& p = sr.recs[i];
-      Engine::SplicePiece& r = recs[i];
-      memset(&r, 0, sizeof(r));
-      r.bit_start = start[i];
-      if (p.stored) {
-        r.stored = 1;
-        r.final = p.final ? 1 : 0;
-        r.len = p.inend - p.instart;
-        r.src = r.len ? slot[s] + (p.src - base) : nullptr;
-      } else {
-        r.nbits = p.bits.nbits;
-        r.src = sr.dev_runs + p.src / 8;
-      }
-    }
-    put(recs, end);
-  }
+  void splice(SpanRecords& sr) override { put(sr.recs, span_positions(sr.recs, pend_bits)); }
   size_t hand_out(bool all, bool to_device, unsigned char** out, size_t* outsize) override {
     const size_t used = (size_t)((pend_bits + 7) / 8), n = all ? used : (size_t)(pend_bits / 8);
     if (to_device) {
@@ -205,25 +188,22 @@ struct DeviceWaveStaging : WaveStaging {
 // caller's partly filled last byte are uploaded, spliced on the device, and the new bytes downloaded
 int device_append_span(const unsigned char* span, size_t spansize, unsigned char* bp, unsigned char** out,
                        size_t* outsize) {
-  std::vector<SpanPiece> pieces;
-  std::vector<unsigned char> raw;
-  if (!bp || !out || !outsize || !parse_span(span, spansize, pieces, raw)) return 1;
+  std::vector<Engine::SpanRecord> recs;
+  if (!bp || !out || !outsize || !parse_span(span, spansize, recs)) return 1;
   const unsigned phase = (*outsize > 0) ? *bp : 0u;  // splice_pieces' bit0
   if (phase > 7) return 1;
-  std::vector<uint64_t> start;
-  const uint64_t end = span_positions(pieces, phase, start);
+  const uint64_t end = span_positions(recs, phase);
   const size_t nbytes = (size_t)((end + 7) / 8);
-  if (pieces.empty() || nbytes == 0) {
+  if (recs.empty() || nbytes == 0) {
     *bp = (unsigned char)(end & 7);
     return 0;
   }
-  std::vector<size_t> at(pieces.size());
+  std::vector<size_t> at(recs.size());
   std::vector<unsigned char> src;
-  for (size_t i = 0; i < pieces.size(); i++) {
-    const SpanPiece& p = pieces[i];
+  for (size_t i = 0; i < recs.size(); i++) {
+    const Engine::SpanRecord& r = recs[i];
     at[i] = src.size();
-    if (p.stored) src.insert(src.end(), raw.begin() + p.instart, raw.begin() + p.inend);
-    else src.insert(src.end(), p.bits.bytes.begin(), p.bits.bytes.end());
+    src.insert(src.end(), r.src, r.src + (r.stored ? r.n : (r.n + 7) / 8));
     src.resize((src.size() + 3) & ~(size_t)3);
   }
   const int dev = Engine::current_device();
@@ -235,17 +215,7 @@ int device_append_span(const unsigned char* span, size_t spansize, unsigned char
   Engine::Lease eng(dev);
   if (!src.empty()) eng->upload(d_src, src.data(), src.size());
   if (phase) eng->upload(d_out, *out + *outsize - 1, 1);
-  std::vector<Engine::SplicePiece> recs(pieces.size());
-  for (size_t i = 0; i < pieces.size(); i++) {
-    Engine::SplicePiece& r = recs[i];
-    memset(&r, 0, sizeof(r));
-    r.bit_start = start[i];
-    r.src = d_src + at[i];
-    r.stored = pieces[i].stored ? 1 : 0;
-    r.final = pieces[i].final ? 1 : 0;
-    r.len = pieces[i].inend - pieces[i].instart;
-    r.nbits = pieces[i].bits.nbits;
-  }
+  for (size_t i = 0; i < recs.size(); i++) recs[i].src = d_src + at[i];
   eng->splice(recs, d_out, ds.stream());
   append_stream(nbytes, phase, out, outsize, [&](unsigned char* dst) { eng->download(d_out, dst, nbytes); });
   ds.release(d_src);

@@ -662,26 +662,21 @@ void append_bytes(const unsigned char* src, size_t n, unsigned char** out, size_
 // Every piece's bit offset follows from a prefix sum over the piece sizes, so the pieces are copied
 // (shifted by their bit phase) in parallel straight into the output buffer; only the bytes shared
 // between neighbouring pieces are merged serially.
-uint64_t span_positions(const std::vector<SpanPiece>& pieces, uint64_t bit0, std::vector<uint64_t>& start) {
-  const size_t np = pieces.size();
-  start.resize(np + 1);
+uint64_t span_positions(std::vector<Engine::SpanRecord>& recs, uint64_t bit0) {
   uint64_t pos = bit0;
-  for (size_t i = 0; i < np; i++) {
-    const SpanPiece& p = pieces[i];
-    start[i] = pos;
-    pos = p.stored ? stored_end(pos, p.inend - p.instart) : pos + p.bits.nbits;
+  for (Engine::SpanRecord& r : recs) {
+    r.bit_start = pos;
+    pos = r.stored ? stored_end(pos, r.n) : pos + r.n;
   }
-  start[np] = pos;
   return pos;
 }
 
-void splice_pieces(const std::vector<SpanPiece>& pieces, const unsigned char* in, unsigned char* bp,
-                   unsigned char** out, size_t* outsize) {
-  const size_t np = pieces.size();
+void splice_pieces(std::vector<Engine::SpanRecord>& recs, unsigned char* bp, unsigned char** out, size_t* outsize) {
+  const size_t np = recs.size();
   uint64_t bit0 = (uint64_t)*outsize * 8;
   if (*bp != 0 && *outsize > 0) bit0 = (uint64_t)(*outsize - 1) * 8 + *bp;
-  std::vector<uint64_t> start;
-  const uint64_t pos = span_positions(pieces, bit0, start);
+  const uint64_t pos = span_positions(recs, bit0);
+  auto end_of = [&](size_t i) { return i + 1 < np ? recs[i + 1].bit_start : pos; };
   const size_t oldsize = *outsize, newsize = (size_t)((pos + 7) / 8);
   append_reserve(newsize - oldsize, out, outsize);  // one append of everything
   unsigned char* o = *out;
@@ -689,19 +684,19 @@ void splice_pieces(const std::vector<SpanPiece>& pieces, const unsigned char* in
   struct Edge { size_t byte; unsigned char v; };
   std::vector<Edge> edges(np * 2 + 2, Edge{(size_t)-1, 0});
   for (size_t i = 0; i < np; i++) {
-    const size_t fb = (size_t)(start[i] / 8), lb = (size_t)(start[i + 1] / 8);
+    const size_t fb = (size_t)(recs[i].bit_start / 8), lb = (size_t)(end_of(i) / 8);
     if (fb >= oldsize && fb < newsize) o[fb] = 0;
     if (lb >= oldsize && lb < newsize) o[lb] = 0;
   }
   parallel_for(np, [&](size_t i) {
-    const SpanPiece& p = pieces[i];
-    const uint64_t sb = start[i], eb = start[i + 1];
+    const Engine::SpanRecord& p = recs[i];
+    const uint64_t sb = p.bit_start, eb = end_of(i);
     if (sb == eb) return;
     Edge& e0 = edges[2 * i];
     Edge& e1 = edges[2 * i + 1];
     if (!p.stored) {
-      const unsigned char* src = p.bits.bytes.data();
-      const uint64_t nb = p.bits.nbits;
+      const unsigned char* src = p.src;
+      const uint64_t nb = p.n;
       const int sh = (int)(sb & 7);
       const size_t fb = (size_t)(sb / 8);
       // destination byte fb + k holds source bits [8k - sh, 8k - sh + 8)
@@ -734,12 +729,12 @@ void splice_pieces(const std::vector<SpanPiece>& pieces, const unsigned char* in
       }
     } else {
       uint64_t q = sb;
-      size_t ip = p.instart;
+      size_t ip = 0;
       bool first = true;
       for (;;) {
         size_t bs = 65535;
-        if (ip + bs > p.inend) bs = p.inend - ip;
-        const bool cur_final = ip + bs >= p.inend;
+        if (ip + bs > p.n) bs = (size_t)p.n - ip;
+        const bool cur_final = ip + bs >= p.n;
         const unsigned hdr = (p.final && cur_final) ? 1u : 0u;  // BFINAL, BTYPE 00
         if (first) {
           // header bits land in the (possibly shared) byte q/8 -- and the byte after it when the
@@ -759,7 +754,7 @@ void splice_pieces(const std::vector<SpanPiece>& pieces, const unsigned char* in
         d[1] = (unsigned char)((bs / 256) % 256);
         d[2] = (unsigned char)(nlen % 256);
         d[3] = (unsigned char)((nlen / 256) % 256);
-        memcpy(d + 4, in + ip, bs);
+        if (bs) memcpy(d + 4, p.src + ip, bs);
         q += 32 + (uint64_t)bs * 8;
         if (cur_final) break;
         ip += bs;

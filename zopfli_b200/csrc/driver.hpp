@@ -31,35 +31,20 @@ struct Piece {
   size_t instart = 0, inend = 0;  // stored blocks: absolute input positions
 };
 
-// A record of a position-independent span (ZopfliB200DeflateSpan / AppendSpan): bits that start at bit
-// offset 0, or stored bytes.
-struct BitString {
-  std::vector<uint8_t> bytes;
-  uint64_t nbits = 0;
-};
-struct SpanPiece {
-  bool stored = false;
-  BitString bits;
-  size_t instart = 0, inend = 0;
-  bool final = false;
-  // where the record's bytes come from (deflate_span_records): for bits, the first bit in the emission of the
-  // runs (SpanRecords::ep); stored, the input position of the payload
-  uint64_t src = 0;
-};
-
 // ZopfliB200DeflateSpan's records of a range of units: the driver's pieces, and the records made of them
-// (maximal runs of compressed pieces as bits, stored pieces as ranges of `stored`, their bytes).  `markers`
-// indexes the pieces that are full-flush markers after units that end at a restart point.  The runs are
-// emitted together (ep, run_bits bits): to the host by span_records_to_host, which fills bits.bytes and
-// `stored`, or by a device compressor into dev_runs, which it owns.
+// (maximal runs of compressed pieces as bits, stored pieces as their payload).  `markers` indexes the pieces
+// that are full-flush markers after units that end at a restart point.  The runs are emitted together (ep,
+// run_bits bits) into one buffer; until point_records (api.hpp) points the records at their bytes, at[i] says
+// where record i's bytes are: a bit record's first bit in that buffer, a stored record's input position.
+// `runs` is that buffer when a compressor's staging made it (WaveStaging::take_records; drop_records frees it).
 struct SpanRecords {
   std::vector<Piece> pieces;
-  std::vector<SpanPiece> recs;
-  std::vector<unsigned char> stored;
+  std::vector<Engine::SpanRecord> recs;
+  std::vector<uint64_t> at;
   std::vector<size_t> markers;
   std::vector<Engine::EmitPiece> ep;
   uint64_t run_bits = 0;
-  unsigned char* dev_runs = nullptr;
+  unsigned char* runs = nullptr;
 };
 
 struct HostTimes { double split = 0, emit = 0, other = 0; };
@@ -120,12 +105,12 @@ uint64_t place_pieces(const std::vector<Piece>& pieces, size_t in_base, unsigned
 uint64_t layout_pieces(const std::vector<Piece>& pieces, size_t in_base, uint64_t bit0, std::vector<Engine::EmitPiece>& ep,
                        std::vector<uint64_t>* unit_bits);
 
-// Where span records go when the first starts at bit0: start[i] for record i, start[n] = the end (returned).
+// Where span records go when the first starts at bit0: fills in every record's bit_start and returns the end.
 // The one placement of records, for the host splice below and the device splice (k_splice).
-uint64_t span_positions(const std::vector<SpanPiece>& pieces, uint64_t bit0, std::vector<uint64_t>& start);
+uint64_t span_positions(std::vector<Engine::SpanRecord>& recs, uint64_t bit0);
 
-void splice_pieces(const std::vector<SpanPiece>& pieces, const unsigned char* in, unsigned char* bp,
-                   unsigned char** out, size_t* outsize);
+// Appends the records, their src in host memory, to a zopfli-style buffer at its bit phase *bp.
+void splice_pieces(std::vector<Engine::SpanRecord>& recs, unsigned char* bp, unsigned char** out, size_t* outsize);
 
 // Grows a zopfli-style buffer by n bytes under its capacity rule (util.h:134-155) and returns where they go.
 unsigned char* append_reserve(size_t n, unsigned char** out, size_t* outsize);

@@ -1427,17 +1427,17 @@ uint8_t* Engine::emit_to_device(const std::vector<EmitPiece>& pieces, uint64_t t
   return out;
 }
 
-void Engine::splice(const std::vector<SplicePiece>& recs, uint8_t* dst, void* after_stream) {
+void Engine::splice(const std::vector<SpanRecord>& recs, uint8_t* dst, void* after_stream) {
   Impl& m = *p_;
   Lane& l = m.lane[0];
   std::lock_guard<std::mutex> g(l.mu);
   CK(cudaSetDevice(m.dev));
   // descriptors, then one 16-byte slot per literal, in one upload
   std::vector<SpliceDesc> d;
-  std::vector<std::pair<size_t, const SplicePiece*>> lits;  // (first descriptor, record)
-  for (const SplicePiece& r : recs) {
+  std::vector<std::pair<size_t, const SpanRecord*>> lits;  // (first descriptor, record)
+  for (const SpanRecord& r : recs) {
     if (r.stored) {
-      uint64_t q = r.bit_start, left = r.len, off = 0;
+      uint64_t q = r.bit_start, left = r.n, off = 0;
       do {  // the sub-blocks of write_stored, one CTA each
         const uint64_t bs = left > 65535 ? 65535 : left;
         left -= bs;
@@ -1448,19 +1448,19 @@ void Engine::splice(const std::vector<SplicePiece>& recs, uint8_t* dst, void* af
       continue;
     }
     if (r.literal) {
-      if (r.nbits > 128) { fprintf(stderr, "zopfli-b200: literal splice record of %llu bits\n", (unsigned long long)r.nbits); abort(); }
+      if (r.n > 128) { fprintf(stderr, "zopfli-b200: literal splice record of %llu bits\n", (unsigned long long)r.n); abort(); }
       lits.push_back({d.size(), &r});
     }
-    for (uint64_t t = 0; t < r.nbits; t += kSpliceTileBits)
-      d.push_back(SpliceDesc{r.bit_start + t, std::min(kSpliceTileBits, r.nbits - t), r.src + t / 8, 0, 0, 0});
+    for (uint64_t t = 0; t < r.n; t += kSpliceTileBits)
+      d.push_back(SpliceDesc{r.bit_start + t, std::min(kSpliceTileBits, r.n - t), r.src + t / 8, 0, 0, 0});
   }
   if (d.empty()) return;
   const size_t desc_b = d.size() * sizeof(SpliceDesc), blob_b = desc_b + lits.size() * 16;
   m.emit_desc.ensure(blob_b + 64);
   std::vector<uint8_t> blob(blob_b, 0);
   for (size_t i = 0; i < lits.size(); i++) {
-    const SplicePiece& r = *lits[i].second;
-    memcpy(blob.data() + desc_b + 16 * i, r.src, (size_t)((r.nbits + 7) / 8));
+    const SpanRecord& r = *lits[i].second;
+    memcpy(blob.data() + desc_b + 16 * i, r.src, (size_t)((r.n + 7) / 8));
     d[lits[i].first].src = (const uint8_t*)m.emit_desc.p + desc_b + 16 * i;
   }
   memcpy(blob.data(), d.data(), desc_b);

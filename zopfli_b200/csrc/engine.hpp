@@ -151,20 +151,23 @@ class Engine {
   // set_input_device_copy) with ISIZE = the input size.  user_stream waits for the result; the caller owns it.
   uint8_t* emit_to_device(const std::vector<EmitPiece>& pieces, uint64_t total_bits, const uint8_t* hdr, int hdr_len,
                           int checksum, void* user_stream, size_t* outsize);
-  // A span record (ZopfliB200AppendSpan's format) placed at an absolute bit position of a device stream:
-  // nbits bits from bit 0 of src, or, stored, the len bytes at src as AddNonCompressedBlock lays them out.  src
-  // is device memory of this context's device (a bit record's 4-byte aligned and readable to its last 4-byte
-  // word), or with `literal` a host buffer of at most 16 bytes (a container header or trailer).
-  struct SplicePiece {
-    uint64_t bit_start, nbits;
-    const uint8_t* src;
-    uint64_t len;
-    uint8_t stored, final, literal, pad;
+  // A record of a position-independent span (ZopfliB200DeflateSpan / AppendSpan): n bits from bit 0 of src, or,
+  // stored, the n bytes at src as AddNonCompressedBlock lays them out.  The record points at its bytes, it owns no
+  // copy; whether src is host or device memory is up to the list's consumer.  bit_start is where span_positions
+  // (driver.hpp) places the record in the stream.
+  struct SpanRecord {
+    bool stored = false, final = false;
+    bool literal = false;      // splice() only: src is a host buffer of at most 16 bytes (a container header or trailer)
+    const uint8_t* src = nullptr;
+    uint64_t n = 0;            // bits of a bit record, bytes of a stored one
+    uint64_t bit_start = 0;
   };
-  // k_splice: writes the records into dst, a device buffer whose bits from the first record's bit_start on are
-  // zero (room for the end position rounded up to 4 bytes), after the work queued on after_stream; blocks until
-  // the bytes are in place.  Long records are cut into tiles here, so that one spreads over many CTAs.
-  void splice(const std::vector<SplicePiece>& recs, uint8_t* dst, void* after_stream);
+  // k_splice: writes the records at their bit_start into dst, a device buffer whose bits from the first record's
+  // bit_start on are zero (room for the end position rounded up to 4 bytes), after the work queued on after_stream;
+  // blocks until the bytes are in place.  src is device memory of this context's device (a bit record's 4-byte
+  // aligned and readable to its last 4-byte word) unless `literal`.  Long records are cut into tiles here, so that
+  // one spreads over many CTAs.
+  void splice(const std::vector<SpanRecord>& recs, uint8_t* dst, void* after_stream);
   // host -> device through the context's threaded pinned staging (synchronous)
   void upload(void* dev_dst, const uint8_t* host_src, size_t nbytes);
   // test seam: symbols [0, n) of buffer `buf` (StoreBuf) from host arrays; n <= input size
